@@ -5,6 +5,7 @@
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W                       (N>1, one rank per GPU, NCCL)
   python bench.py --impl reference ...                                 (the reference's algorithm on host CPU cores)
+  python bench.py ... --dump-outputs DIR                               (also write the last timed step's results as .npy)
 
 A "step" = one training pass of the hot path over one batch of synthetic nuScenes-shaped frames:
 reader (voxelize + PillarFeatureNet) -> sparse ResNet-18 -> ASPP -> CenterHead -> CenterPoint loss -> backward
@@ -20,6 +21,8 @@ import subprocess
 import sys
 import threading
 import time
+
+import numpy as np
 
 import torch
 
@@ -40,11 +43,11 @@ def peaks():
             p = json.load(fh)
         return dict(hbm=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sust=p.get("bf16_tflops_sustained", p["bf16_tflops"]), src="measured")
     except Exception:
-        return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+        return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -199,7 +202,35 @@ def main_reference(args):
     print(json.dumps(line))
 
 
-# ------------------------------------------------------------------------------------------------- B200 arm
+def dump_outputs(out_dir, model, loss, logs):
+    """The loss, logged terms and updated model state (after AdamW) of a training step: one .npy per array, float32
+    (integer counters float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss}
+
+    def flatten(name, v):
+        if torch.is_tensor(v) or isinstance(v, (int, float)):
+            arrays[name] = v
+        elif isinstance(v, dict):
+            for k, e in v.items():
+                flatten("%s.%s" % (name, k), e)
+        elif isinstance(v, (list, tuple)):
+            for i, e in enumerate(v):
+                flatten("%s.%d" % (name, i), e)
+
+    flatten("logs", logs)
+    for k, v in model.state_dict().items():
+        arrays["state." + k] = v
+    total = 0
+    for name, v in arrays.items():
+        v = v.detach().cpu() if torch.is_tensor(v) else torch.tensor(v)
+        a = v.numpy().astype(np.float32 if v.is_floating_point() else np.float64)
+        total += a.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    assert total <= 64 << 20, "dumped outputs exceed 64 MB (%d bytes)" % total
+
+
+# ------------------------------------------------------------------------------------------------- GPU arm
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -213,6 +244,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--sync-bn", action="store_true", help="SyncBatchNorm semantics (reference default sync_batchnorm: True) instead of local BN")
     ap.add_argument("--voxelize-sweep", action="store_true", help="also report voxelizer GB/s over batch sizes")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's loss, logged terms and updated model state as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return main_reference(args)
@@ -262,12 +295,15 @@ def main():
     from pillarnext_b200.parallel import BucketedGradAllReduce, default_buckets
     reducer = BucketedGradAllReduce(default_buckets(model))     # head | neck | backbone+reader, overlapped with the backward
 
+    last = {}
+
     def step(ex):
-        loss, _ = model(ex)
+        loss, logs = model(ex)
         loss.backward()
         reducer.finish()
         opt.step()
         opt.zero_grad(set_to_none=True)
+        last["loss"], last["logs"] = loss, logs
         return loss
 
     copy_stream = torch.cuda.Stream(device=dev)
@@ -343,6 +379,8 @@ def main():
     ms = timed(args.steps, False)
     launches = ops.LAUNCHES - l0
     clocks = sampler.finish() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, last["loss"], last["logs"])
     timed(2 * nb + 2, True)             # untimed: every distinct batch once through the copy stream's allocator pool and the read-back path
     ms_e2e = timed(args.steps, True)
     # host-side enqueue time of one step (python + autograd + ctypes launches), no synchronisation inside
@@ -356,25 +394,13 @@ def main():
     value = frames_total / (ms / 1e3)
     e2e = frames_total / (ms_e2e / 1e3)
 
-    # ---- roofline of the dominant kernel family (tcgen05 implicit GEMM + weight-gradient GEMM), one probe step with
+    # ---- roofline of the dominant kernel family (wgmma implicit GEMM + weight-gradient GEMM), one probe step with
     #      CUDA events around every launch on the launching stream
     ops.PROFILE = []
     step(resident[0])
     torch.cuda.synchronize()
     prof, ops.PROFILE = ops.PROFILE, None
     agg = {}
-    if rank == 0 and os.path.isdir(os.path.join(ROOT, "gpurun_out")):
-        per = {}
-        for kind, flops, nb_, a, b, tag in prof:
-            d = per.setdefault(kind + ":" + tag, [0, 0.0, 0.0])
-            d[0] += 1
-            d[1] += a.elapsed_time(b)
-            d[2] += flops
-        rows = sorted(((v[1], k, v[0], v[2]) for k, v in per.items()), reverse=True)
-        with open(os.path.join(ROOT, "gpurun_out", "probe_gemm_calls.txt"), "w") as fh:
-            fh.write("# ms_total  calls  TFLOP/s  kind:shape   (one probe step, CUDA events per launch)\n")
-            for t, k, c, f in rows:
-                fh.write("%9.3f %4d %8.1f  %s\n" % (t, c, f / (t * 1e-3) / 1e12 if t > 0 else 0, k))
     for kind, flops, nb_, a, b, _tag in prof:
         d = agg.setdefault(kind, [0.0, 0.0, 0])
         d[0] += flops
@@ -385,9 +411,9 @@ def main():
     gemm_fl = sum(v[0] for v in agg.values())
     ig = [sum(agg.get(k, [0.0, 0.0, 0])[i] for k in ("igemm", "igemm_win")) for i in range(3)]
     ig[1] = max(ig[1], 1e-9)
-    roof = {"bound": "tensor", "kernel": "igemm_kernel + igemm_win_kernel (tcgen05 implicit GEMM: TMA gather4 / TMA window producers; fwd+dgrad)",
+    roof = {"bound": "tensor", "kernel": "igemm_kernel + igemm_win_kernel (wgmma implicit GEMM: cp.async row gather / TMA window producers; fwd+dgrad)",
             "achieved": ig[0] / (ig[1] * 1e-3) / 1e12, "peak": pk["tf_sust"], "unit": "TFLOP/s",
-            "frac": ig[0] / (ig[1] * 1e-3) / 1e12 / pk["tf_sust"], "traffic": None, "traffic_detail": None, "peak_source": pk["src"] + " (sustained bf16)",
+            "frac": ig[0] / (ig[1] * 1e-3) / 1e12 / pk["tf_sust"], "traffic": None, "traffic_detail": None, "peak_source": pk["src"] + " (bf16)",
             "launches": ig[2], "flops_per_step": ig[0], "share_of_step": ig[1] / (ms / args.steps),
             "wgrad": {"achieved": agg["wgrad"][0] / (agg["wgrad"][1] * 1e-3) / 1e12, "launches": agg["wgrad"][2],
                       "share_of_step": agg["wgrad"][1] / (ms / args.steps)} if "wgrad" in agg else None,
@@ -419,7 +445,7 @@ def main():
                 "dtype": "bf16", "data": "synthetic",
                 "config": {"workload": workload(sel, args.points, args.frames), "name": args.config, "global_batch": args.frames * world,
                            "parallelism": "dp%d (frames sharded, bucketed NCCL gradient all-reduce overlapped with the backward, %s BatchNorm)" % (world, "synchronised" if (args.sync_bn and world > 1) else "local"),
-                           "l2": "per-step activation working set (GBs) >> 126 MB L2; 4 distinct input batches rotated",
+                           "l2": "per-step activation working set (GBs) >> 50 MB L2; 4 distinct input batches rotated",
                            "timed_step": "reader+backbone+neck+head fwd, loss, bwd, grad all-reduce (N>1), AdamW",
                            "gc": "Python cyclic GC collected before and disabled inside each timed region"},
                 "e2e": {"value": e2e, "unit": "frames/s", "h2d_bytes_per_step": nbytes(host_raw[0]), "d2h_bytes_per_step": 4,
@@ -427,6 +453,7 @@ def main():
                         "pipeline": "inside the timed region every step: pinned-host -> device copy of its inputs = points + raw ground-truth "
                                     "boxes (side stream, overlapping the previous step), label assignment on the GPU (pnx_assign_labels), "
                                     "and a 4-byte loss read-back (async copy to pinned memory + event, consumed one step late)"},
+                "gpu": torch.cuda.get_device_name(dev), "peak_memory_gb": torch.cuda.max_memory_allocated(dev) / 1e9,
                 "gpu_launches": launches, "host_enqueue_ms_per_step": host_ms, "clocks": clocks, "roofline": roof, "voxelize": vox, "cpu_baseline": cpu}
         print(json.dumps(line))
         if world > 1 and nccl_log and os.path.exists(nccl_log):
@@ -462,7 +489,7 @@ def traffic_from_profile(kernel_prefixes, path=None):
 def voxelize_roofline(dev, sel, pk):
     """Index-generation voxelizer (pnx_voxelize: V1-V2) swept over frames per launch on the selected config's point
     clouds.  Algorithmic bytes (SURVEY 8d): 24*N + 4*Nv + 12*P; the headline entry is the largest launch (>= 64 MB of
-    algorithmic bytes, input larger than the 126 MB L2 so every timed iteration streams from HBM)."""
+    algorithmic bytes, input larger than the 50 MB L2 so every timed iteration streams from HBM)."""
     from pillarnext_b200 import ops, synth
     cfg, n = sel["cfg"], sel["points"]
     nbase = 16 if n <= 60000 else 4

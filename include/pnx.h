@@ -1,4 +1,4 @@
-/* pnx.h -- C-ABI of libpnx.so, the B200 (sm_100a) hot path of PillarNeXt-B.
+/* pnx.h -- C-ABI of libpnx.so, the H100 (sm_90a) hot path of PillarNeXt-B.
  *
  * Boundary rules (SURVEY.md section 8b): extern "C", plain pointers and sizes, no torch types.
  * The caller owns every buffer (device memory unless stated), kernels never allocate and never
@@ -156,9 +156,9 @@ int pnx_nbr_table(const int* dst_coords, const int* n_dst_ptr, int cap, const ui
 int pnx_scatter_dense(const void* feat, const int* coords, const int* n_ptr, int cap, int channels,
                       int batch, int u, int v, void* canvas, int gather, cudaStream_t stream);
 
-/* ---------------------------------------------------------------- tcgen05 gather implicit GEMM
+/* ---------------------------------------------------------------- wgmma gather implicit GEMM
  * out[m, n] = sum_{t<taps} sum_{c<Cin} A[nbr(m,t), c] * W[t, n, c]  (+ bias[n]) (relu)
- *   A       [a_rows, lda] bf16 (a_rows = rows really allocated: the TMA map carries the true extent)
+ *   A       [a_rows, lda] bf16 (a_rows = rows really allocated; every gathered row index must be below it)
  *   W       [taps, Cout, Cin] bf16 (packed, K-major)
  *   nbr(m,t): nbr[m*taps+t] if nbr != NULL; computed from the dense geometry if dense != 0
  *             (m -> (b, y, x) over Hout x Wout; source pixel (y*mul + r*dil - pad, x*mul + s*dil - pad)
@@ -184,7 +184,7 @@ int pnx_igemm(const void* A, long long lda, long long a_rows, int M, int taps, i
  * pnx_bn_bwd_apply is then called with relu = 0 on g.  Same trailing arguments on pnx_conv3x3_win. */
 /* nseg > 1 selects the fp32-grade SPLIT mode (see "split rows" below): every value is a sum of bf16 PIECES, A rows
  * hold piece p of channel c at column p*a_lo_off + c, W is packed [taps, Cout, pieces*Cin] = [piece 0 | piece 1 | ..],
- * and the K loop accumulates nseg (A piece, W piece) segments into the same fp32 TMEM accumulator in the order given
+ * and the K loop accumulates nseg (A piece, W piece) segments into the same fp32 register accumulator in the order given
  * by seg_code (4 bits per segment: (A piece << 2) | W piece; callers put the smallest products first).
  * addend_fp32 = 1: `addend` is fp32 [M, ld_add] (requires out_fp32).  nseg = 1, seg_code = 0, a_lo_off = 0,
  * addend_fp32 = 0: the production bf16 path. */
@@ -209,7 +209,7 @@ int pnx_conv3x3_win(const void* A, long long lda, int B, int H, int W, int Cin, 
                     const float* bnr_shift, const float* bnr_mean, const float* bnr_invstd, double* bnr_red, int bnr_C,
                     int sm_count, cudaStream_t stream);
 
-/* ---------------------------------------------------------------- tcgen05 weight gradient
+/* ---------------------------------------------------------------- wgmma weight gradient
  * dW[t, x, y] += sum_m X[m, x] * Y[g(m,t), y]   (fp32, red.global.add; zero dW first)
  * X = direct operand (output gradient; layer input for ConvTranspose2d, shuffle=1), Y = operand read through
  * the neighbour map: nbr[m*taps+t] if nbr != NULL, else the dense geometry (as pnx_igemm), else row m (taps==1,

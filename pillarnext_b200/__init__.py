@@ -1,4 +1,4 @@
-"""pillarnext_b200 -- B200 (sm_100a) native hot path of PillarNeXt-B behind the reference's det3d module API.
+"""pillarnext_b200 -- H100 (sm_90a) native hot path of PillarNeXt-B behind the reference's det3d module API.
 
 csrc/ + libpnx.so : hand-written CUDA kernels behind the C-ABI in include/pnx.h
 ops.py            : device-buffer plumbing (torch) -> C-ABI calls

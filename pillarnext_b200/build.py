@@ -1,4 +1,4 @@
-"""Build libpnx.so (the C-ABI CUDA library, include/pnx.h) in-tree with nvcc for sm_100a.
+"""Build libpnx.so (the C-ABI CUDA library, include/pnx.h) in-tree with nvcc for sm_90a (H100).
 
 `python -m pillarnext_b200.build` or `__graft_entry__.build()`.  Cross-compiles without a GPU.
 """
@@ -13,8 +13,8 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libpnx.so")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-         "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _sources():
@@ -52,7 +52,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(one, _sources()))
-    cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [NVCC, "-shared", "-o", OUT] + objs + ARCH + ["-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

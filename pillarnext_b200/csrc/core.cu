@@ -62,29 +62,6 @@ int pnx_encode_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, u
   return PNX_OK;
 }
 
-// 2-D map for cp.async.bulk.tensor tile::gather4: box = [64 channels x 1 row], 128B swizzle
-int pnx_encode_tmap_gather_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                                uint64_t row_stride_bytes) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) {
-    pnx_set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-    return PNX_ERR_CUDA;
-  }
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {row_stride_bytes};
-  cuuint32_t box[2] = {64, 1};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    pnx_set_error("cuTensorMapEncodeTiled(gather) failed: CUresult %d (rows=%llu cols=%llu stride=%llu)", (int)r,
-                  (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)row_stride_bytes);
-    return PNX_ERR_CUDA;
-  }
-  return PNX_OK;
-}
-
 int pnx_encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3],
                             const uint32_t box[4]) {
   EncodeTiledFn fn = get_encode_fn();

@@ -1,4 +1,4 @@
-// igemm.cu -- gather implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// igemm.cu -- gather implicit-GEMM convolution on wgmma tensor cores (sm_90a).
 //
 // One engine for every convolution on the path (rows B1-B3, N1, H1 of SURVEY.md section 8a; their
 // data-gradients too):   out[m, n] = sum_t sum_c  A[nbr(m,t), c] * W[t, n, c]   (+bias)(relu)
@@ -8,15 +8,11 @@
 //     centerhead.py:35-46,108-114): rows = pixels of a channels-last image, nbr computed from geometry
 //     (zero padding = absent neighbour), ConvTranspose2d k2 s2 (centerhead.py:26-27) = one GEMM with
 //     N = 4*Cout and a pixel-shuffle store.
-// Pipeline per CTA (persistent over 128-row tiles, one CTA per SM):
-//   warp 0        : TMA (cp.async.bulk.tensor) producer of the weight tile  B[BN x 64]  (SWIZZLE_128B)
-//   warp 1        : single-thread tcgen05.mma issue, fp32 accumulators in TMEM (2 sets x BN columns)
-//   PW warps      : gather producers: TMA tile::gather4 requests (4 arbitrary rows x 128 B each) into the same
-//                   128B-swizzled K-major layout; row index -1 (absent neighbour) = out of bounds = zero fill
-//   2 warps       : index warps: row indices of the next tile ([tap][row] table in shared memory)
-//   4 or 8 warps  : epilogue: tcgen05.ld -> bias/relu/addend -> bf16|fp32 coalesced store through a swizzled slab,
-//                   fused BatchNorm statistics (per-channel sum / sum of squares, fp64 accumulate)
-#include "pnx_common.cuh"
+// CTA = 3 warpgroups, persistent over 128-row tiles: warpgroup 0 writes the gathered row of every (tap, row) of a tile
+// into shared memory, then per K stage loads the weight tile by TMA and gathers the 128 A rows with 16-byte cp.async
+// (index -1 = zero fill) into the 128B-swizzled layout; warpgroups 1-2 each run wgmma on 64 rows into registers and
+// apply the epilogue (gemm_epilogue.cuh).
+#include "gemm_epilogue.cuh"
 
 namespace {
 
@@ -26,16 +22,6 @@ struct IgemmParams {
   int M, T, Cin, w_rows_per_tap;
   const int* nbr;
   int dense, Hout, Wout, Hin, Win, kw, mul, dil, pad;
-  void* out;
-  long long ldc;
-  int out_fp32;
-  const float* bias;
-  double* stats;
-  int stats_C, stats_mod;
-  int stats_direct;  // deterministic mode: per-warp partials go straight to the fp64 accumulators (no fp32 shared-memory stage)
-  int shuffle, relu;
-  const __nv_bfloat16* addend;  // optional [M, ld_add] bf16 added before the store (gradient accumulation)
-  long long ld_add;
   // fp32-grade "split" mode: every value is the sum of P bf16 PIECES (P = 2: hi + lo, 16 mantissa bits; P = 3:
   // hi + mid + lo, 24 bits).  A rows hold piece p of channel c at column p * a_lo_off + c, W rows are
   // [piece 0 (Cin) | piece 1 (Cin) | ...]; the K loop runs nseg (A piece, W piece) segments into the same fp32
@@ -44,43 +30,27 @@ struct IgemmParams {
   // accumulator would lose most of their low bits.  nseg = 1 (piece 0 x piece 0): plain bf16.
   int nseg, a_lo_off;
   unsigned long long seg_code;  // 4 bits per segment, in execution order: (A piece << 2) | W piece
-  const float* addend_f32;      // fp32 addend (split mode: gradients are accumulated in fp32)
-  // Fused BatchNorm-backward reduction (bf16 staged store only): this GEMM produces dy, the gradient of y = relu(bn(raw)).
-  // The epilogue re-creates the ReLU gate from `raw` with the forward affine, stores g = dy * gate instead of dy and
-  // accumulates red[c] += sum g, red[C + c] += sum g * xhat (xhat = (raw - mean) * invstd) -- the reduce pass of the
-  // BatchNorm backward (elementwise.cu bn_bwd_reduce_kernel) without a separate sweep over dy and raw.
-  const __nv_bfloat16* bnr_raw;
-  long long bnr_ld;
+  pnx::EpiParams epi;
+  int out_fp32;
+  const float* bias;
   const float* bnr_scale; const float* bnr_shift; const float* bnr_mean; const float* bnr_invstd;
   double* bnr_red;
   int bnr_C;
 };
 
-__device__ __forceinline__ void unpack_bf16x8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const float2 t = __bfloat1622float2(h[k]);
-    f[2 * k] = t.x;
-    f[2 * k + 1] = t.y;
-  }
-}
+constexpr int kThreads = 384;           // producer warpgroup + two consumer warpgroups
+constexpr uint32_t kABytes = 128 * 128;  // one A stage: 128 rows x 64 bf16
+constexpr int kProducerRegs = 56, kConsumerRegs = 224;
 
-// threads = TMA warp + MMA warp + PW gather warps + 2 index warps + EW epilogue warps.
-constexpr uint32_t kABytes = 128 * 128;
-
-// MT = 128-row tiles per CTA iteration (1 everywhere: MT = 2, one weight stage against two A tiles, was measured
-// slower -- the single accumulator set exposes the epilogue and only 3 stages fit).
-template <int BN, int MT, int EW>
+template <int BN>
 struct Cfg {
   static constexpr uint32_t kBBytes = BN * 128;
-  static constexpr uint32_t kAStage = MT * kABytes;
-  static constexpr int kStagesRaw = (192 * 1024 - (EW - 4) * 4096) / (int)(kAStage + kBBytes);
-  static constexpr int kStagesCap = 8;
-  static constexpr int kStages = kStagesRaw > kStagesCap ? kStagesCap : kStagesRaw;
-  static constexpr int kAccSets = 512 / (MT * BN) >= 2 ? 2 : 1;  // TMEM accumulator sets (2 = epilogue overlaps the next tile)
-  static constexpr int kTblSlots = MT == 1 ? 2 : 3;  // ring of per-tile index tables [9 taps][128 rows] (smem budget: 3 for MT = 2)
-  static constexpr size_t kSmem = 1024 + (size_t)kStages * (kAStage + kBBytes) + kTblSlots * 128 * 9 * 4 + 256 + EW * 4096 + 2 * BN * 4 + BN * 4 + 4 * BN * 4;
+  static constexpr int kTbl = 128 * 9;  // ints of the per-tile index table [tap][row]
+  static constexpr int kFixed = 1024 + kTbl * 4 + 256 + (2 * pnx::kEpiWarps + 5) * BN * 4;
+  static constexpr int kStagesRaw = (227 * 1024 - kFixed) / (int)(kABytes + kBBytes);
+  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
+  static constexpr size_t kSmem = (size_t)kFixed + (size_t)kStages * (kABytes + kBBytes);
+  static_assert(kStages >= 3, "pipeline depth");
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
 
@@ -88,233 +58,70 @@ __device__ __forceinline__ void named_bar_sync(int id, int n) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
 
-__device__ __forceinline__ float colsum32(float (&v)[32]) {
-  const uint32_t lane = pnx::lane_id();
-#pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int k = 0; k < off; ++k) {
-      float send = upper ? v[k] : v[k + off];
-      float keep = upper ? v[k + off] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  return v[0];
-}
-
-// EW = epilogue warps: 4 (one per TMEM lane quarter) or 8 (two per quarter, alternating 64-column block pairs) for the
-// short-K wide-N layers whose epilogue is longer than their MMA loop
-// F = compile-time feature set of the epilogue (the epilogue shares the instruction cache with the producer / MMA warps:
-// the lean production variant must not carry the rarely used paths -- measured 10-25 % on the 3x3 layers):
-//   0 production: bf16 (or unstaged fp32) output, bias / ReLU / bf16 addend / forward BatchNorm statistics / pixel shuffle
-//   1 + fused BatchNorm-backward reduce (bnr_*)          2 fp32-grade paths: staged fp32 store + statistics, fp32 addend
-template <int BN, int PW, int MT, int SPLIT, int EW, int F>
-__global__ void __launch_bounds__(64 + PW * 32 + 64 + EW * 32, 1) igemm_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap amap,
-                                                                  IgemmParams p) {
-  using C = Cfg<BN, MT, EW>;
-  constexpr uint32_t kAStage = C::kAStage;
-  constexpr int kAccSets = C::kAccSets;
-  constexpr int kTbl = 128 * 9;  // ints per tile index table
-  constexpr int kTblSlots = C::kTblSlots;
-  constexpr int kProducerWarps = PW;
-  constexpr int kIndexWarps = 2;  // compute the gathered row indices of the next tile while the gather warps issue
-  constexpr int kThreadsTotal = 64 + PW * 32 + kIndexWarps * 32 + EW * 32;
-  constexpr int kEpiWarp0 = 2 + PW + kIndexWarps;
+template <int BN, int F>
+__global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constant__ CUtensorMap wmap, IgemmParams p) {
+  using C = Cfg<BN>;
   constexpr int kStages = C::kStages;
-  static_assert(PW <= MT * SPLIT * kStages, "gather warps must not outnumber the stage slots (mbarrier parity)");
-  static_assert(SPLIT == 1 || SPLIT == 2 || SPLIT == 4, "warps per 128-row gather");
   constexpr uint32_t kBBytes = C::kBBytes;
-  constexpr int kColBlk = BN >= 32 ? 32 : 16;
-  constexpr int kNumCB = BN / kColBlk;
+  constexpr int kTbl = C::kTbl;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
-  uint8_t* sB = smem + (size_t)kStages * kAStage;
+  uint8_t* sB = smem + (size_t)kStages * kABytes;
   int* s_idx = reinterpret_cast<int*>(sB + (size_t)kStages * kBBytes);  // [T][128 rows] gathered row index, -1 = absent
-  uint64_t* full = reinterpret_cast<uint64_t*>(s_idx + kTblSlots * kTbl);
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_idx + kTbl);
   uint64_t* empty = full + kStages;
-  uint64_t* tfull = empty + kStages;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* tbl_full = tempty + 2;            // index warps -> gather warps (ring of tile tables)
-  uint64_t* tbl_empty = tbl_full + kTblSlots;  // gather warps -> index warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tbl_empty + kTblSlots);
-  float* s_tr = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);   // [4 warps][4 KB] store staging slabs
-  float* s_stat = s_tr + EW * 1024;                                                      // [2][BN] per-channel sum / sumsq (smem atomics)
-  float* s_bias = s_stat + 2 * BN;                                                // [BN] bias of this CTA's column block
-  float* s_bnc = s_bias + BN;                                                     // [4][BN] fused BN-backward: scale, shift, mean, invstd
+  float* s_stat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);  // [8 warps][2][BN] per-channel sums
+  float* s_bias = s_stat + pnx::kEpiWarps * 2 * BN;                                  // [BN] bias of this CTA's columns
+  float* s_bnc = s_bias + BN;                                                        // [4][BN] fused BN-backward affine
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
+  const int n0 = blockIdx.y * BN;
 
-  if (warp == 0 && pnx::elect_one()) {
+  if (threadIdx.x == 0) {
     pnx::tma_prefetch_desc(&wmap);
-    pnx::tma_prefetch_desc(&amap);
     for (int s = 0; s < kStages; ++s) {
-      pnx::mbar_init(&full[s], 1 + MT * SPLIT);  // weight producer + SPLIT gather warps per A tile (all arrive with expect_tx)
-      pnx::mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      pnx::mbar_init(&tfull[a], 1);
-      pnx::mbar_init(&tempty[a], EW);
-    }
-    for (int a = 0; a < kTblSlots; ++a) {
-      pnx::mbar_init(&tbl_full[a], kIndexWarps);
-      pnx::mbar_init(&tbl_empty[a], kProducerWarps);
+      pnx::mbar_init(&full[s], 1 + 128);  // weight TMA (expect_tx) + the 128 gathering threads (cp.async arrive)
+      pnx::mbar_init(&empty[s], 8);       // one arrival per consumer warp
     }
     pnx::fence_barrier_init();
   }
-  if (warp == 1) pnx::tmem_alloc<512>(tmem_slot);
   if (p.bias)
-    for (int c = threadIdx.x; c < BN; c += blockDim.x) s_bias[c] = p.bias[blockIdx.y * BN + c];
-  for (int c = threadIdx.x; c < 2 * BN; c += blockDim.x) s_stat[c] = 0.f;
+    for (int c = threadIdx.x; c < BN; c += blockDim.x) s_bias[c] = p.bias[n0 + c];
+  for (int c = threadIdx.x; c < pnx::kEpiWarps * 2 * BN; c += blockDim.x) s_stat[c] = 0.f;
   if (F == 1)
     for (int c = threadIdx.x; c < BN; c += blockDim.x) {
-      const int gc = blockIdx.y * BN + c;
+      const int gc = n0 + c;
       s_bnc[c] = p.bnr_scale[gc]; s_bnc[BN + c] = p.bnr_shift[gc]; s_bnc[2 * BN + c] = p.bnr_mean[gc]; s_bnc[3 * BN + c] = p.bnr_invstd[gc];
     }
-  pnx::tc_fence_before();
   __syncthreads();
-  pnx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_tiles = (p.M + 127) >> 7;
-  const int num_pairs = (num_tiles + MT - 1) / MT;  // CTA iterations (groups of MT tiles)
-  const int n0 = blockIdx.y * BN;
   const int kpt = p.Cin >> 6;
   const int num_k = p.T * kpt * p.nseg;
 
-  if (warp == 0) {
-    // ---------------------------------------------------------------- TMA weight producer
-    if (pnx::elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int pt = blockIdx.x; pt < num_pairs; pt += gridDim.x) {
-        for (int kc = 0; kc < num_k; ++kc) {
-          const int ccx = kc / p.T, t = kc - ccx * p.T;  // chunk outer, tap inner: consecutive stages re-read overlapping rows
-          const int seg = ccx / kpt, cc = ccx - seg * kpt;
-          const int wpiece = (int)((p.seg_code >> (4 * seg)) & 3ull);
-          pnx::mbar_wait(&empty[stage], phase ^ 1);
-          pnx::mbar_arrive_expect_tx(&full[stage], kBBytes);
-          pnx::tma_load_2d(&wmap, &full[stage], sB + (size_t)stage * kBBytes, cc * 64 + wpiece * p.Cin, t * p.w_rows_per_tap + n0);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    if (pnx::elect_one()) {
-      constexpr uint32_t idesc = pnx::make_idesc_bf16(128, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int pt = blockIdx.x; pt < num_pairs; pt += gridDim.x) {
-        pnx::mbar_wait(&tempty[acc], acc_phase ^ 1);
-        pnx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * (MT * BN);
-        for (int kc = 0; kc < num_k; ++kc) {
-          pnx::mbar_wait(&full[stage], phase);
-          pnx::tc_fence_after();
-          const uint32_t a_base = pnx::smem_u32(sA + (size_t)stage * kAStage);
-          const uint32_t b_base = pnx::smem_u32(sB + (size_t)stage * kBBytes);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t db = pnx::make_smem_desc_sw128(b_base + k * 32, 0, 1024);
-#pragma unroll
-            for (int h = 0; h < MT; ++h) {
-              const uint64_t da = pnx::make_smem_desc_sw128(a_base + h * kABytes + k * 32, 0, 1024);
-              pnx::umma_f16(d_tmem + h * BN, da, db, idesc, (kc > 0 || k > 0) ? 1u : 0u);
-            }
-          }
-          pnx::umma_commit(&empty[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        pnx::umma_commit(&tfull[acc]);
-        if (++acc == kAccSets) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp < 2 + kProducerWarps) {
-    // ---------------------------------------------------------------- A gather producers (TMA tile::gather4)
-    // One request = 4 arbitrary rows x 128 B of A, landed in the 128B-swizzled K-major tile; lane l of the issuing
-    // warp owns rows 4l..4l+3 of the 128-row tile, so one warp instruction fills a whole stage.  Absent neighbours
-    // are row index -1 = out of bounds = zero fill.  The (chunk, tap) stages go round-robin over the producer warps
-    // (a warp sustains ~8 B/clk of requests, the SM ~50 B/clk: tools/gather4_rate.cu).  Row indices come from the
-    // index warps' table of the tile ([tap][row], one LDS.128 per request).
-    const int pw = warp - 2;
-    uint32_t g_base = 0;
-    uint32_t tcount = 0;  // tiles consumed by this CTA so far (table ring position)
-    for (int pt = blockIdx.x; pt < num_pairs; pt += gridDim.x) {
-#pragma unroll
-      for (int h = 0; h < MT; ++h) {
-        const uint32_t c = tcount + h;
-        pnx::mbar_wait(&tbl_full[c % kTblSlots], (c / kTblSlots) & 1u);
-      }
-      // item i = (stage g, tile half h, part s of the 32 requests), global count over iterations, belongs to warp
-      // i % PW: a warp's consecutive items are PW / (MT*SPLIT) <= kStages stages apart, so it can never be two phases
-      // ahead of an `empty` barrier.  SPLIT > 1 shortens the serial request issue of one stage (32 x ~66 clk).
-      constexpr int kParts = MT * SPLIT, kLanes = 32 / SPLIT;
-      const uint32_t i_base = g_base * kParts;
-      for (int it = (int)((pw + kProducerWarps - i_base % kProducerWarps) % kProducerWarps); it < num_k * kParts; it += kProducerWarps) {
-        const int kc = it / kParts, hs = it - kc * kParts;
-        const int h = hs / SPLIT, part = hs - h * SPLIT;
-        const int ccx = kc / p.T, t = kc - ccx * p.T;  // chunk outer, tap inner: consecutive stages re-read overlapping rows
-        const int seg = ccx / kpt, cc = ccx - seg * kpt;
-        const int acol = cc * 64 + (int)((p.seg_code >> (4 * seg + 2)) & 3ull) * p.a_lo_off;
-        const uint32_t g = g_base + (uint32_t)kc;
-        const uint32_t stage = g % (uint32_t)kStages, phase = (g / (uint32_t)kStages) & 1u;
-        const int* tbl = s_idx + ((tcount + h) % kTblSlots) * kTbl;
-        const int l4 = part * kLanes + lane;  // request index within the tile: rows 4*l4 .. 4*l4+3
-        int4 rows = make_int4(-1, -1, -1, -1);
-        if (lane < kLanes) rows = *reinterpret_cast<const int4*>(tbl + t * 128 + 4 * l4);
-        pnx::mbar_wait(&empty[stage], phase ^ 1);
-        if (lane == 0) pnx::mbar_arrive_expect_tx(&full[stage], kABytes / SPLIT);
-        __syncwarp();
-        if (lane < kLanes)
-          pnx::tma_gather4(&amap, &full[stage], pnx::smem_u32(sA + (size_t)stage * kAStage) + h * kABytes + l4 * 512, acol,
-                           rows.x, rows.y, rows.z, rows.w);
-      }
-      g_base += (uint32_t)num_k;
-      __syncwarp();
-      if (lane == 0) {
-#pragma unroll
-        for (int h = 0; h < MT; ++h) pnx::mbar_arrive(&tbl_empty[(tcount + h) % kTblSlots]);
-      }
-      tcount += MT;
-    }
-  } else if (warp < 2 + kProducerWarps + kIndexWarps) {
-    // ---------------------------------------------------------------- index warps: gathered row of (row r, tap t) for the
-    // NEXT tiles while the gather warps work on the current ones (ring of tile tables).  Thread i owns rows i, i + 64.
-    const int itid = threadIdx.x - 64 - kProducerWarps * 32;
+  if (wg == 0) {
+    // ---------------------------------------------------------------- producer
+    pnx::regs_dealloc<kProducerRegs>();
+    const int ptid = threadIdx.x;
+    const int sub = ptid & 7, rsub = ptid >> 3;  // a warp instruction copies 4 whole 128-byte rows
     const int hw = p.Hout * p.Wout;
-    const float inv_hw = 1.0f / (float)hw, inv_w = 1.0f / (float)p.Wout;
-    uint32_t tcount = 0;
-    for (int pt = blockIdx.x; pt < num_pairs; pt += gridDim.x) {
-#pragma unroll 1
-      for (int h = 0; h < 2 * MT; ++h) {
-        const uint32_t c = tcount + (h >> 1);
-        int* tbl = s_idx + (c % kTblSlots) * kTbl;   // table of tile c: [tap][row]
-        if ((h & 1) == 0) pnx::mbar_wait(&tbl_empty[c % kTblSlots], ((c / kTblSlots) & 1u) ^ 1u);
-        const int r = itid + 64 * (h & 1);
-        const int m = (pt * MT + (h >> 1)) * 128 + r;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      named_bar_sync(1, 128);  // every thread is done reading the previous tile's table
+      {
+        const int r = ptid;
+        const int m = tile * 128 + r;
         if (m >= p.M) {
-          for (int t = 0; t < p.T; ++t) tbl[t * 128 + r] = -1;
+          for (int t = 0; t < p.T; ++t) s_idx[t * 128 + r] = -1;
         } else if (p.nbr) {
           const int* src = p.nbr + (size_t)m * p.T;
-          for (int t = 0; t < p.T; ++t) tbl[t * 128 + r] = src[t];
+          for (int t = 0; t < p.T; ++t) s_idx[t * 128 + r] = src[t];
         } else if (p.dense) {
-          int b, rem, y, x;
-          if (m < (1 << 24)) {
-            b = __float2int_rz(__int2float_rn(m) * inv_hw);
-            rem = m - b * hw;
-            if (rem < 0) { --b; rem += hw; } else if (rem >= hw) { ++b; rem -= hw; }
-            y = __float2int_rz(__int2float_rn(rem) * inv_w);
-            x = rem - y * p.Wout;
-            if (x < 0) { --y; x += p.Wout; } else if (x >= p.Wout) { ++y; x -= p.Wout; }
-          } else {
-            b = m / hw; rem = m - b * hw; y = rem / p.Wout; x = rem - y * p.Wout;
-          }
+          const int b = m / hw, rem = m - b * hw, y = rem / p.Wout, x = rem - y * p.Wout;
           const int base = b * p.Hin;
           int t = 0;
           for (int rr = 0; t < p.T; ++rr) {
@@ -322,354 +129,100 @@ __global__ void __launch_bounds__(64 + PW * 32 + 64 + EW * 32, 1) igemm_kernel(c
             const bool yok = yi >= 0 && yi < p.Hin;
             for (int ss = 0; ss < p.kw && t < p.T; ++ss, ++t) {
               const int xi = x * p.mul + ss * p.dil - p.pad;
-              tbl[t * 128 + r] = (yok && xi >= 0 && xi < p.Win) ? (base + yi) * p.Win + xi : -1;
+              s_idx[t * 128 + r] = (yok && xi >= 0 && xi < p.Win) ? (base + yi) * p.Win + xi : -1;
             }
           }
         } else {
-          tbl[r] = m;
-        }
-        if (h & 1) {
-          __syncwarp();
-          if (lane == 0) pnx::mbar_arrive(&tbl_full[c % kTblSlots]);
+          s_idx[r] = m;
         }
       }
-      tcount += MT;
+      named_bar_sync(1, 128);
+      for (int kc = 0; kc < num_k; ++kc) {
+        const int ccx = kc / p.T, t = kc - ccx * p.T;  // chunk outer, tap inner: consecutive stages re-read overlapping rows
+        const int seg = ccx / kpt, cc = ccx - seg * kpt;
+        const int wpiece = (int)((p.seg_code >> (4 * seg)) & 3ull);
+        const int acol = cc * 64 + (int)((p.seg_code >> (4 * seg + 2)) & 3ull) * p.a_lo_off + sub * 8;
+        pnx::mbar_wait(&empty[stage], phase ^ 1);
+        if (ptid == 0) {
+          pnx::mbar_arrive_expect_tx(&full[stage], kBBytes);
+          pnx::tma_load_2d(&wmap, &full[stage], sB + (size_t)stage * kBBytes, cc * 64 + wpiece * p.Cin, t * p.w_rows_per_tap + n0);
+        }
+        const uint32_t a_dst = pnx::smem_u32(sA + (size_t)stage * kABytes);
+        const int* tbl = s_idx + t * 128;
+#pragma unroll
+        for (int it = 0; it < 8; ++it) {
+          const int r = rsub + 16 * it;
+          const int g = tbl[r];
+          const __nv_bfloat16* src = p.A + (long long)(g < 0 ? 0 : g) * p.lda + acol;
+          pnx::cp_async_16(a_dst + pnx::sw128_offset(r, sub), src, g < 0 ? 0u : 16u);
+        }
+        pnx::cp_async_mbar_arrive(&full[stage]);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
     }
   } else {
-    // ---------------------------------------------------------------- epilogue (4 warps = 128 TMEM lanes)
-    // The column-block loop is deliberately NOT unrolled: the unrolled form was >170 KB of SASS and the epilogue
-    // ran out of the instruction cache (stall_no_inst); per-channel statistics live in shared memory.
-    const int quarter = warp & 3, group = (warp - kEpiWarp0) >> 2;
-    int acc = 0, ti = 0;
-    uint32_t acc_phase = 0;
-    float* st_sum = s_stat;
-    float* st_sq = s_stat + BN;
-    uint8_t* slab = reinterpret_cast<uint8_t*>(s_tr) + (warp - kEpiWarp0) * 4096;
-    const int hw = p.Hout * p.Wout;
-    // the staged (coalesced) store also serves the ConvTranspose2d pixel-shuffle when a 64-column pair of blocks is one
-    // output pixel (BN % 64 == 0, bf16): the 128-byte row of the slab goes to pixel (2y + q/2, 2x + q%2)
-    // F = 0 / 1 only ever see bf16 outputs (the host dispatch sends fp32 outputs to F = 2): always staged when BN % 64 == 0
-    constexpr bool kHasUnstaged = (BN % 64 != 0) || F == 2;   // the per-thread store path is compiled only where reachable
-    const bool staged = (BN % 64 == 0) && !(F == 2 && p.shuffle);
-    for (int pt = blockIdx.x; pt < num_pairs; pt += gridDim.x) {
-      while (!pnx::mbar_try_wait(&tfull[acc], acc_phase)) __nanosleep(64);  // leave the issue slots to the producers
-      pnx::tc_fence_after();
-#pragma unroll 1
-      for (int h = 0; h < MT; ++h) {
-      const int tile = pt * MT + h;
-      if (tile >= num_tiles) break;
-      const int m = tile * 128 + quarter * 32 + lane;
-      const bool active = m < p.M;
-      long long out_row = m;
-      int sh_b = 0, sh_y = 0, sh_x = 0;
-      if (p.shuffle && active) {
-        sh_b = m / hw;
-        const int rem = m - sh_b * hw;
-        sh_y = rem / p.Wout;
-        sh_x = rem - sh_y * p.Wout;
+    // ---------------------------------------------------------------- consumers: wgmma + epilogue
+    pnx::regs_alloc<kConsumerRegs>();
+    const int half = wg - 1;  // rows [64 * half, 64 * half + 64) of every tile
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int prev = 0;
+      for (int kc = 0; kc < num_k; ++kc) {
+        pnx::mbar_wait(&full[stage], phase);
+        pnx::fence_proxy_async_smem();  // the cp.async rows were written through the generic proxy; wgmma reads async
+        pnx::wgmma_fence();
+        pnx::fence_acc(acc);
+        const uint32_t a_base = pnx::smem_u32(sA + (size_t)stage * kABytes) + half * 64 * 128;
+        const uint32_t b_base = pnx::smem_u32(sB + (size_t)stage * kBBytes);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          pnx::Wgmma<BN, 0, 0>::mma(acc, pnx::make_smem_desc_sw128(a_base + k * 32, 16, 1024),
+                                    pnx::make_smem_desc_sw128(b_base + k * 32, 16, 1024), (kc > 0 || k > 0) ? 1u : 0u);
+        pnx::wgmma_commit();
+        pnx::wgmma_wait<1>();  // the previous stage's MMAs are done: release it
+        if (kc > 0 && lane == 0) pnx::mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
-#pragma unroll 1
-      for (int cb = 0; cb < kNumCB; ++cb) {
-        if (EW == 8 && (((cb >> 1) + ti) & 1) != group) continue;  // the other warp of this lane quarter takes it
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (acc * MT + h) * BN + cb * kColBlk;
-        if (kColBlk == 32) pnx::tmem_ld_32x32b_x32(taddr, r);
-        else pnx::tmem_ld_32x32b_x16(taddr, r);
-        pnx::tmem_ld_wait();
-        const int ncol0 = n0 + cb * kColBlk;
-        float v[32];
-#pragma unroll
-        for (int k = 0; k < kColBlk; ++k) v[k] = __uint_as_float(r[k]);
-#pragma unroll
-        for (int k = kColBlk; k < 32; ++k) v[k] = 0.f;
-        if (p.bias) {
-#pragma unroll
-          for (int k = 0; k < kColBlk; k += 4) {
-            const float4 bq = *reinterpret_cast<const float4*>(s_bias + cb * kColBlk + k);  // smem broadcast
-            v[k] += bq.x; v[k + 1] += bq.y; v[k + 2] += bq.z; v[k + 3] += bq.w;
-          }
-        }
-        if (p.addend && active) {
-          const uint4* ap = reinterpret_cast<const uint4*>(p.addend + (long long)m * p.ld_add + ncol0);
-#pragma unroll
-          for (int k = 0; k < kColBlk / 8; ++k) {
-            const uint4 u = __ldg(ap + k);
-            const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 f = __bfloat1622float2(h2[j]);
-              v[8 * k + 2 * j] += f.x;
-              v[8 * k + 2 * j + 1] += f.y;
-            }
-          }
-        }
-        if (F == 2 && p.addend_f32 && active) {
-          const float4* ap = reinterpret_cast<const float4*>(p.addend_f32 + (long long)m * p.ld_add + ncol0);
-#pragma unroll
-          for (int k = 0; k < kColBlk / 4; ++k) {
-            const float4 u = __ldg(ap + k);
-            v[4 * k] += u.x; v[4 * k + 1] += u.y; v[4 * k + 2] += u.z; v[4 * k + 3] += u.w;
-          }
-        }
-        if (p.relu) {
-#pragma unroll
-          for (int k = 0; k < kColBlk; ++k) v[k] = fmaxf(v[k], 0.f);
-        }
-        if (F == 2 && staged) {
-          // fp32 output: one 32-column block = [32 rows x 128 B] slab, flushed as full 128-byte lines
-#pragma unroll
-          for (int k = 0; k < 8; ++k)
-            *reinterpret_cast<float4*>(slab + lane * 128 + ((k ^ (lane & 7)) << 4)) =
-                make_float4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-          __syncwarp();
-          const int ch = lane & 7;
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int row = it * 4 + (lane >> 3);
-            const long long mr = (long long)tile * 128 + quarter * 32 + row;
-            if (mr < p.M) {
-              const float4 val = *reinterpret_cast<const float4*>(slab + row * 128 + ((ch ^ (row & 7)) << 4));
-              *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + mr * p.ldc + ncol0 + ch * 4) = val;
-            }
-          }
-          if (p.stats) {
-            // lane = column of this 32-column block: sum the stored fp32 values over the tile's valid rows
-            const long long row0 = (long long)tile * 128 + quarter * 32;
-            const int nrows = (int)max((long long)0, min((long long)32, (long long)p.M - row0));
-            float s0 = 0.f, q0 = 0.f;
-            for (int row = 0; row < nrows; ++row) {
-              const float f = *reinterpret_cast<const float*>(slab + row * 128 + (((lane >> 2) ^ (row & 7)) << 4) + (lane & 3) * 4);
-              s0 += f;
-              q0 = fmaf(f, f, q0);
-            }
-            // fp32-grade mode: the per-warp partials go straight to the fp64 accumulators.  Four warps adding fp32 partials
-            // into one shared-memory word in arrival order perturbs the statistics at 1e-7, which now and then flips a ReLU
-            // gate / a scatter_max winner downstream and moves a gradient by 1e-3 from one run to the next (measured);
-            // fp64 adds differ at 1e-16 whatever the order.
-            const int ch = (n0 + cb * 32 + lane) % p.stats_mod;
-            atomicAdd(&p.stats[ch], (double)s0);
-            atomicAdd(&p.stats[p.stats_C + ch], (double)q0);
-          }
-          __syncwarp();
-        } else if (staged) {
-          // bf16 output: two 32-column blocks are staged per warp as a [32 rows x 128 B] slab (16-byte chunks
-          // XOR-swizzled by row), then written back 8 lanes per row = full 128-byte lines; the BatchNorm statistics
-          // of the 64 columns are read back from the slab (lane = column pair, 32 conflict-free LDS)
-          const int half = cb & 1;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint4 pk = make_uint4(pnx::pack_bf16x2(v[8 * k], v[8 * k + 1]), pnx::pack_bf16x2(v[8 * k + 2], v[8 * k + 3]),
-                                        pnx::pack_bf16x2(v[8 * k + 4], v[8 * k + 5]), pnx::pack_bf16x2(v[8 * k + 6], v[8 * k + 7]));
-            *reinterpret_cast<uint4*>(slab + lane * 128 + (((half * 4 + k) ^ (lane & 7)) << 4)) = pk;
-          }
-          if (half == 1) {
-            __syncwarp();
-            const int ch = lane & 7;
-            const long long row0 = (long long)tile * 128 + quarter * 32;
-            // pixel-shuffle: output row of this lane's own input row m (quadrant q = 64-column pair), fetched by shuffle below
-            long long sh_base = 0;
-            if (p.shuffle) {
-              const int q = (ncol0 - 32) >> 6;
-              sh_base = ((long long)(sh_b * 2 * p.Hout + 2 * sh_y + (q >> 1))) * (2 * p.Wout) + 2 * sh_x + (q & 1);
-            }
-            if (F == 1) {
-              // fused BatchNorm-backward reduce: lane = (row group, 8-channel chunk); gate from raw, g = dy * gate
-              const int c8 = (cb - 1) * 32 + ch * 8;  // first of this lane's 8 columns inside the CTA's column block
-              float sg[8], sgx[8], csc[8], csh[8], cmu[8], cis[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                sg[k] = sgx[k] = 0.f;
-                csc[k] = s_bnc[c8 + k]; csh[k] = s_bnc[BN + c8 + k]; cmu[k] = s_bnc[2 * BN + c8 + k]; cis[k] = s_bnc[3 * BN + c8 + k];
-              }
-              uint4 rws[8];
-#pragma unroll
-              for (int it = 0; it < 8; ++it) {  // the eight raw loads of this lane are in flight together
-                const int row = it * 4 + (lane >> 3);
-                rws[it] = make_uint4(0u, 0u, 0u, 0u);
-                if (row0 + row < p.M) rws[it] = __ldg(reinterpret_cast<const uint4*>(p.bnr_raw + (row0 + row) * p.bnr_ld + n0 + c8));
-              }
-#pragma unroll
-              for (int it = 0; it < 8; ++it) {
-                const int row = it * 4 + (lane >> 3);
-                if (row0 + row < p.M) {
-                  float d[8], rw[8];
-                  unpack_bf16x8(*reinterpret_cast<const uint4*>(slab + row * 128 + ((ch ^ (row & 7)) << 4)), d);
-                  unpack_bf16x8(rws[it], rw);
-#pragma unroll
-                  for (int k = 0; k < 8; ++k) {
-                    const float g = fmaf(rw[k], csc[k], csh[k]) > 0.f ? d[k] : 0.f;
-                    d[k] = g;
-                    sg[k] += g;
-                    sgx[k] = fmaf(g, (rw[k] - cmu[k]) * cis[k], sgx[k]);
-                  }
-                  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (row0 + row) * p.ldc + (ncol0 - 32) + ch * 8) =
-                      make_uint4(pnx::pack_bf16x2(d[0], d[1]), pnx::pack_bf16x2(d[2], d[3]), pnx::pack_bf16x2(d[4], d[5]), pnx::pack_bf16x2(d[6], d[7]));
-                }
-              }
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {  // the four lanes that share a channel chunk (lane ^ 8, lane ^ 16)
-                sg[k] += __shfl_xor_sync(0xffffffffu, sg[k], 8);
-                sgx[k] += __shfl_xor_sync(0xffffffffu, sgx[k], 8);
-                sg[k] += __shfl_xor_sync(0xffffffffu, sg[k], 16);
-                sgx[k] += __shfl_xor_sync(0xffffffffu, sgx[k], 16);
-              }
-              if (lane < 8) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                  atomicAdd(&st_sum[c8 + k], sg[k]);
-                  atomicAdd(&st_sq[c8 + k], sgx[k]);
-                }
-              }
-            } else {
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int row = it * 4 + (lane >> 3);
-              const long long orow = p.shuffle ? __shfl_sync(0xffffffffu, sh_base, row) : row0 + row;
-              if (row0 + row < p.M) {
-                const uint4 val = *reinterpret_cast<const uint4*>(slab + row * 128 + ((ch ^ (row & 7)) << 4));
-                const int ocol = p.shuffle ? 0 : ncol0 - 32;
-                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + orow * p.ldc + ocol + ch * 8) = val;
-              }
-            }
-            }
-            if (p.stats) {
-              const int nrows = (int)min((long long)32, (long long)p.M - row0);  // rows past M hold bias-only garbage
-              float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-              const int cpc = lane >> 2, cps = (lane & 3) * 4;
-              // full 32-row blocks (all but the ragged tile edge): unrolled so the 32 LDS are in flight together
-              if (nrows == 32) {
-#pragma unroll
-                for (int row = 0; row < 32; ++row) {
-                  const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(slab + row * 128 + ((cpc ^ (row & 7)) << 4) + cps);
-                  const float2 f = __bfloat1622float2(h2);
-                  s0 += f.x; s1 += f.y;
-                  q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-                }
-              } else {
-                for (int row = 0; row < nrows; ++row) {
-                  const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(slab + row * 128 + ((cpc ^ (row & 7)) << 4) + cps);
-                  const float2 f = __bfloat1622float2(h2);
-                  s0 += f.x; s1 += f.y;
-                  q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-                }
-              }
-              const int c0 = (cb - 1) * 32 + 2 * lane;  // columns of this pair of blocks owned by this lane
-              if (p.stats_direct) {   // order-insensitive (fp64) accumulation, see pnx_set_deterministic
-                const int ch0 = (n0 + c0) % p.stats_mod, ch1 = (n0 + c0 + 1) % p.stats_mod;
-                atomicAdd(&p.stats[ch0], (double)s0); atomicAdd(&p.stats[ch1], (double)s1);
-                atomicAdd(&p.stats[p.stats_C + ch0], (double)q0); atomicAdd(&p.stats[p.stats_C + ch1], (double)q1);
-              } else {
-                atomicAdd(&st_sum[c0], s0); atomicAdd(&st_sum[c0 + 1], s1);
-                atomicAdd(&st_sq[c0], q0); atomicAdd(&st_sq[c0 + 1], q1);
-              }
-            }
-            __syncwarp();
-          }
-        } else if constexpr (kHasUnstaged) {
-          if (!p.out_fp32) {
-#pragma unroll
-            for (int k = 0; k < kColBlk; ++k) v[k] = pnx::bf16_round(v[k]);
-          }
-          if (active) {
-            int col = ncol0;
-            if (p.shuffle) {
-              const int q = ncol0 >> 6;
-              out_row = ((long long)(sh_b * 2 * p.Hout + 2 * sh_y + (q >> 1))) * (2 * p.Wout) + 2 * sh_x + (q & 1);
-              col = ncol0 & 63;
-            }
-            if (p.out_fp32) {
-              float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + out_row * p.ldc + col);
-#pragma unroll
-              for (int k = 0; k < kColBlk / 4; ++k) dst[k] = make_float4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-            } else {
-              uint4* dst = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + out_row * p.ldc + col);
-#pragma unroll
-              for (int k = 0; k < kColBlk / 8; ++k)
-                dst[k] = make_uint4(pnx::pack_bf16x2(v[8 * k], v[8 * k + 1]), pnx::pack_bf16x2(v[8 * k + 2], v[8 * k + 3]),
-                                    pnx::pack_bf16x2(v[8 * k + 4], v[8 * k + 5]), pnx::pack_bf16x2(v[8 * k + 6], v[8 * k + 7]));
-            }
-          }
-          if (p.stats) {
-            float a[32];
-#pragma unroll
-            for (int k = 0; k < 32; ++k) {
-              v[k] = active ? v[k] : 0.f;
-              a[k] = v[k];
-            }
-            const float s1 = colsum32(a);
-#pragma unroll
-            for (int k = 0; k < 32; ++k) v[k] *= v[k];
-            const float s2 = colsum32(v);
-            if (lane < kColBlk) {  // lane c owns column c of this warp's accumulators
-              if (F == 2 || p.stats_direct) {  // fp32-grade / deterministic mode: order-insensitive fp64 accumulation
-                const int ch = (n0 + cb * kColBlk + lane) % p.stats_mod;
-                atomicAdd(&p.stats[ch], (double)s1);
-                atomicAdd(&p.stats[p.stats_C + ch], (double)s2);
-              } else {
-                atomicAdd(&st_sum[cb * kColBlk + lane], s1);
-                atomicAdd(&st_sq[cb * kColBlk + lane], s2);
-              }
-            }
-          }
-        }
-      }
-      }  // h
-      pnx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) pnx::mbar_arrive(&tempty[acc]);
-      if (++acc == kAccSets) { acc = 0; acc_phase ^= 1; }
-      ++ti;
+      pnx::wgmma_wait<0>();
+      pnx::fence_acc(acc);
+      if (lane == 0) pnx::mbar_arrive(&empty[prev]);
+      const long long row0 = (long long)tile * 128;
+      pnx::gemm_epilogue<BN, F>(acc, p.epi, row0, (int)min((long long)128, (long long)p.M - row0), half, n0, s_bias, s_stat, s_bnc);
     }
-    if (p.stats && F != 2 && !p.stats_direct) {
-      named_bar_sync(2, EW * 32);  // the epilogue warps
-      for (int c = threadIdx.x - (kThreadsTotal - EW * 32); c < BN; c += EW * 32) {
-        const int ch = (n0 + c) % p.stats_mod;
-        atomicAdd(&p.stats[ch], (double)st_sum[c]);
-        atomicAdd(&p.stats[p.stats_C + ch], (double)st_sq[c]);
-      }
-    } else if (F == 1) {
-      named_bar_sync(2, EW * 32);
-      for (int c = threadIdx.x - (kThreadsTotal - EW * 32); c < BN; c += EW * 32) {
-        atomicAdd(&p.bnr_red[n0 + c], (double)st_sum[c]);
-        atomicAdd(&p.bnr_red[p.bnr_C + n0 + c], (double)st_sq[c]);
-      }
-    }
+    named_bar_sync(2, 256);
+    pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, threadIdx.x - 128, 256);
   }
-
-  pnx::tc_fence_before();
-  __syncthreads();
-  pnx::tc_fence_after();
-  if (warp == 1) pnx::tmem_dealloc<512>(tmem_base);
 }
 
-template <int BN, int PW, int MT, int SPLIT, int EW, int F>
-int launch_igemm_f(const CUtensorMap& wmap, const CUtensorMap& amap, const IgemmParams& p, int n_blocks, int sm_count,
-                   cudaStream_t stream) {
+template <int BN, int F>
+int launch_igemm_f(const CUtensorMap& wmap, const IgemmParams& p, int n_blocks, int sm_count, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    PNX_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, PW, MT, SPLIT, EW, F>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)Cfg<BN, MT, EW>::kSmem));
+    PNX_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN>::kSmem));
     attr_set = true;
   }
   const int num_tiles = (p.M + 127) / 128;
-  const int num_pairs = (num_tiles + MT - 1) / MT;
   int gx = sm_count / n_blocks;
   if (gx < 1) gx = 1;
-  if (gx > num_pairs) gx = num_pairs;
+  if (gx > num_tiles) gx = num_tiles;
   dim3 grid(gx, n_blocks);
-  igemm_kernel<BN, PW, MT, SPLIT, EW, F><<<grid, 64 + PW * 32 + 64 + EW * 32, Cfg<BN, MT, EW>::kSmem, stream>>>(wmap, amap, p);
+  igemm_kernel<BN, F><<<grid, kThreads, Cfg<BN>::kSmem, stream>>>(wmap, p);
   PNX_CHECK_LAUNCH();
   return PNX_OK;
 }
 
-template <int BN, int PW, int MT, int SPLIT, int EW>
-int launch_igemm(const CUtensorMap& wmap, const CUtensorMap& amap, const IgemmParams& p, int n_blocks, int sm_count,
-                 cudaStream_t stream) {
-  if (p.bnr_raw) {
-    if constexpr (BN % 64 == 0) return launch_igemm_f<BN, PW, MT, SPLIT, EW, 1>(wmap, amap, p, n_blocks, sm_count, stream);
+template <int BN>
+int launch_igemm(const CUtensorMap& wmap, const IgemmParams& p, int n_blocks, int sm_count, cudaStream_t stream) {
+  if (p.epi.bnr_raw) {
+    if constexpr (BN % 64 == 0) return launch_igemm_f<BN, 1>(wmap, p, n_blocks, sm_count, stream);
   }
-  if (p.out_fp32 || p.addend_f32) return launch_igemm_f<BN, PW, MT, SPLIT, EW, 2>(wmap, amap, p, n_blocks, sm_count, stream);
-  return launch_igemm_f<BN, PW, MT, SPLIT, EW, 0>(wmap, amap, p, n_blocks, sm_count, stream);
+  if (p.out_fp32 || p.epi.addend_f32) return launch_igemm_f<BN, 2>(wmap, p, n_blocks, sm_count, stream);
+  return launch_igemm_f<BN, 0>(wmap, p, n_blocks, sm_count, stream);
 }
 
 }  // namespace
@@ -709,7 +262,7 @@ extern "C" int pnx_igemm(const void* A, long long lda, long long a_rows, int M, 
   PNX_CHECK_ARG(nbr || dense || taps == 1, "taps > 1 needs a neighbour table or dense geometry");
   PNX_CHECK_ARG(!shuffle || (block_n % 64 == 0 || 64 % block_n == 0), "shuffle store needs 64-channel groups");
   if (stats) PNX_CHECK_ARG(stats_C > 0 && stats_mod > 0, "stats_C/stats_mod");
-  if (sm_count <= 0) sm_count = 148;
+  if (sm_count <= 0) sm_count = 132;
   IgemmParams p;
   p.A = (const __nv_bfloat16*)A;
   p.lda = lda;
@@ -717,14 +270,18 @@ extern "C" int pnx_igemm(const void* A, long long lda, long long a_rows, int M, 
   p.nbr = nbr; p.dense = dense;
   p.Hout = Hout > 0 ? Hout : 1; p.Wout = Wout > 0 ? Wout : 1; p.Hin = Hin; p.Win = Win;
   p.kw = kw > 0 ? kw : 1; p.mul = mul; p.dil = dil; p.pad = pad;
-  p.out = out; p.ldc = ldc; p.out_fp32 = out_fp32; p.bias = bias;
-  p.stats = stats; p.stats_C = stats_C; p.stats_mod = stats_mod > 0 ? stats_mod : 1 << 30;
-  p.stats_direct = g_pnx_deterministic;
-  p.shuffle = shuffle; p.relu = relu;
-  p.addend = addend_fp32 ? nullptr : (const __nv_bfloat16*)addend;
-  p.addend_f32 = addend_fp32 ? (const float*)addend : nullptr;
-  p.ld_add = ld_add;
+  p.out_fp32 = out_fp32; p.bias = bias;
+  pnx::EpiParams& e = p.epi;
+  e.out = out; e.ldc = ldc; e.has_bias = bias != nullptr; e.relu = relu;
+  e.stats = stats; e.stats_C = stats_C; e.stats_mod = stats_mod > 0 ? stats_mod : 1 << 30;
+  e.stats_direct = g_pnx_deterministic;
+  e.shuffle = shuffle; e.Hout = p.Hout; e.Wout = p.Wout;
+  e.addend = addend_fp32 ? nullptr : (const __nv_bfloat16*)addend;
+  e.addend_f32 = addend_fp32 ? (const float*)addend : nullptr;
+  e.ld_add = ld_add;
+  e.bnr_raw = (const __nv_bfloat16*)bnr_raw; e.bnr_ld = bnr_ld;
   PNX_CHECK_ARG(!(addend && shuffle), "addend is not supported with the pixel-shuffle store");
+  PNX_CHECK_ARG(!addend || (ld_add % 2 == 0 && (reinterpret_cast<uintptr_t>(addend) & 7) == 0), "addend: even row stride, 8-byte aligned");
   PNX_CHECK_ARG(nseg >= 1 && nseg <= 9, "nseg in [1,9]");
   int a_pieces = 1, w_pieces = 1;
   for (int sgi = 0; sgi < nseg; ++sgi) {
@@ -737,10 +294,10 @@ extern "C" int pnx_igemm(const void* A, long long lda, long long a_rows, int M, 
   PNX_CHECK_ARG(a_pieces == 1 || (a_lo_off >= Cin && a_lo_off % 64 == 0 && (a_pieces - 1) * a_lo_off + Cin <= lda), "split mode: a_lo_off");
   PNX_CHECK_ARG(!addend_fp32 || out_fp32, "an fp32 addend needs an fp32 output");
   p.nseg = nseg; p.a_lo_off = (int)a_lo_off; p.seg_code = (unsigned long long)seg_code;
-  p.bnr_raw = (const __nv_bfloat16*)bnr_raw; p.bnr_ld = bnr_ld; p.bnr_scale = bnr_scale; p.bnr_shift = bnr_shift;
+  p.bnr_scale = bnr_scale; p.bnr_shift = bnr_shift;
   p.bnr_mean = bnr_mean; p.bnr_invstd = bnr_invstd; p.bnr_red = bnr_red; p.bnr_C = bnr_C;
   if (bnr_raw) {
-    PNX_CHECK_ARG(!out_fp32 && !shuffle && !stats && block_n % 64 == 0, "fused BN-backward reduce: bf16 staged store without forward statistics");
+    PNX_CHECK_ARG(!out_fp32 && !shuffle && !stats && block_n % 64 == 0, "fused BN-backward reduce: bf16 output without forward statistics");
     PNX_CHECK_ARG(bnr_scale && bnr_shift && bnr_mean && bnr_invstd && bnr_red && bnr_C == Cout && bnr_ld % 8 == 0 &&
                       (reinterpret_cast<uintptr_t>(bnr_raw) & 15) == 0, "fused BN-backward reduce: arguments");
   }
@@ -749,31 +306,15 @@ extern "C" int pnx_igemm(const void* A, long long lda, long long a_rows, int M, 
   int rc = pnx_encode_tmap_2d_bf16(&wmap, Wpacked, (uint64_t)taps * Cout, (uint64_t)wcols, (uint64_t)wcols * 2,
                                    (uint32_t)block_n, 64);
   if (rc) return rc;
-  // A as a 2-D tensor [a_rows, Cin] for tile::gather4 (box = one 64-channel row); index -1 = absent neighbour = out of
-  // range = zero fill.  The map carries the TRUE row count: a map that claims 2^31 rows (256 GB) makes the gather
-  // instruction fault ("warp illegal address") for some placements of A near the end of a mapping -- measured with
-  // tools/tma_tail_probe.py; with the exact extent it never does.
-  CUtensorMap amap;
   PNX_CHECK_ARG(a_rows >= 1 && a_rows < 0x7fffffffLL, "a_rows = number of rows of A");
-  rc = pnx_encode_tmap_gather_bf16(&amap, A, (uint64_t)a_rows, (uint64_t)((a_pieces - 1) * a_lo_off + Cin), (uint64_t)lda * 2);
-  if (rc) return rc;
   const int n_blocks = Cout / block_n;
   switch (block_n) {
-    case 16: return launch_igemm<16, 8, 1, 1, 4>(wmap, amap, p, n_blocks, sm_count, stream);
-    case 32: return launch_igemm<32, 8, 1, 1, 4>(wmap, amap, p, n_blocks, sm_count, stream);
-    case 64: return launch_igemm<64, 8, 1, 1, 4>(wmap, amap, p, n_blocks, sm_count, stream);
-    case 128:
-      if (taps * (Cin / 64) * nseg <= 4) return launch_igemm<128, 4, 1, 2, 8>(wmap, amap, p, n_blocks, sm_count, stream);
-      return launch_igemm<128, 8, 1, 2, 4>(wmap, amap, p, n_blocks, sm_count, stream);
-    case 192:  // short K (1x1 convs of the head): the epilogue of 192 columns outlasts the MMA loop -> 8 epilogue warps
-      if (taps * (Cin / 64) * nseg <= 9) return launch_igemm<192, 4, 1, 2, 8>(wmap, amap, p, n_blocks, sm_count, stream);
-      return launch_igemm<192, 8, 1, 2, 4>(wmap, amap, p, n_blocks, sm_count, stream);
-    case 256:
-      // (MT = 2, two tiles per weight stage, measured slower on every layer of the step: exposed epilogue of the single
-      // accumulator set and only 3 stages -- not instantiated)
-      // short K (1x1 convs, ConvTranspose2d): the 256-column epilogue outlasts the <= 4-stage MMA loop -> 8 epilogue warps
-      if (taps * (Cin / 64) * nseg <= 4) return launch_igemm<256, 4, 1, 2, 8>(wmap, amap, p, n_blocks, sm_count, stream);
-      return launch_igemm<256, 8, 1, 4, 4>(wmap, amap, p, n_blocks, sm_count, stream);
+    case 16: return launch_igemm<16>(wmap, p, n_blocks, sm_count, stream);
+    case 32: return launch_igemm<32>(wmap, p, n_blocks, sm_count, stream);
+    case 64: return launch_igemm<64>(wmap, p, n_blocks, sm_count, stream);
+    case 128: return launch_igemm<128>(wmap, p, n_blocks, sm_count, stream);
+    case 192: return launch_igemm<192>(wmap, p, n_blocks, sm_count, stream);
+    case 256: return launch_igemm<256>(wmap, p, n_blocks, sm_count, stream);
     default:
       pnx_set_error("pnx_igemm: unsupported block_n %d (16/32/64/128/192/256)", block_n);
       return PNX_ERR_ARG;

@@ -1,16 +1,16 @@
-// igemm_win.cu -- dense 3x3 'same' convolution (stride 1, dilation 1) on tcgen05 with the im2col folded into TMA.
+// igemm_win.cu -- dense 3x3 'same' convolution (stride 1, dilation 1) on wgmma with the im2col folded into TMA.
 //
 // The gather engine (igemm.cu) re-reads every input row once per tap: for the head's 336x336 maps with few output
 // channels (reference det3d/models/heads/centerhead.py:35-46,108-114 and their data gradients) that makes the
-// L2->SM fabric the limit (~5-6 TB/s measured).  Here one M tile = 128 consecutive pixels of ONE image row, and for
+// L2->SM fabric the limit.  Here one M tile = 128 consecutive pixels of ONE image row, and for
 // each 64-channel K chunk and each kernel row r the producer issues ONE 4-D TMA load of the 130-pixel window
 // (x0-1 .. x0+128, y+r-1) -- out-of-image pixels are zero-filled by the TMA unit, i.e. the padding -- into a
-// 128B-swizzled smem buffer.  The three horizontal taps s = 0,1,2 are the SAME buffer read through UMMA descriptors
-// whose start address is shifted by s rows (s*128 bytes, matrix base offset = s): 3 window loads feed 9 taps,
+// 128B-swizzled smem buffer.  The three horizontal taps s = 0,1,2 are the SAME buffer read through wgmma descriptors
+// whose start address is shifted by s rows (s*128 bytes): 3 window loads feed 9 taps,
 // cutting the activation traffic 2.9x, and there are no gather warps at all (one thread issues every load).
-//   warp 0: TMA producer (A windows, 4-D map [C, W, H, B]; weight tiles, 2-D map)   warp 1: MMA issuer
-//   warps 2..9: epilogue (bias, ReLU, bf16 coalesced store through a swizzled slab, BatchNorm statistics)
-#include "pnx_common.cuh"
+//   warpgroup 0: TMA producer (A windows, 4-D map [C, W, H, B]; weight tiles, 2-D map)
+//   warpgroups 1-2: wgmma on 64 pixels each, fp32 register accumulators, epilogue (gemm_epilogue.cuh)
+#include "gemm_epilogue.cuh"
 
 extern int g_pnx_deterministic;  // igemm.cu (pnx_set_deterministic)
 
@@ -19,46 +19,29 @@ namespace {
 struct WinParams {
   int B, H, W, XC;          // XC = ceil(W / 128) tiles per image row
   int Cin, Cout_total;
-  __nv_bfloat16* out;
-  long long ldc;
   const float* bias;
-  double* stats;
-  int stats_C;
-  int stats_direct;
-  int relu;
   int base_off_mode;        // 1: descriptor base offset = (start >> 7) & 7 (PTX ISA), 0: leave 0
-  // fused BatchNorm-backward reduction (see igemm.cu IgemmParams): this conv produces dy of y = relu(bn(raw))
-  const __nv_bfloat16* bnr_raw;
-  long long bnr_ld;
+  pnx::EpiParams epi;
   const float* bnr_scale; const float* bnr_shift; const float* bnr_mean; const float* bnr_invstd;
   double* bnr_red;
   int bnr_C;
 };
 
-__device__ __forceinline__ void unpack_bf16x8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const float2 t = __bfloat1622float2(h[k]);
-    f[2 * k] = t.x;
-    f[2 * k + 1] = t.y;
-  }
-}
-
+constexpr int kThreads = 384;
 constexpr uint32_t kWinRows = 130;
 constexpr uint32_t kWinBytes = kWinRows * 128;     // bytes written by one window load
 constexpr uint32_t kWinSlot = 17 * 1024;           // 1024-aligned slot
 
 // WS = weights stationary: for Cin = 64 the nine [BN x 64] weight tiles (9*BN*128 B) are loaded once per CTA and stay in
 // shared memory; a stage is then only the activation window.  Without it every 128-pixel tile re-fetches all nine
-// tiles (216 KB at BN = 192 against 50 KB of windows) and the kernel is bound by L2->SM traffic at ~50 % MMA issue.
+// tiles (216 KB at BN = 192 against 50 KB of windows).
 template <int BN, bool WS>
 struct WCfgWin {
   static constexpr uint32_t kBTap = BN * 128;
   static constexpr uint32_t kWBytes = WS ? 9 * kBTap : 0;
   static constexpr uint32_t kStageBytes = WS ? kWinSlot : kWinSlot + 3 * kBTap;
-  static constexpr int kFixed = 1024 + 256 + 8 * 4096 + 3 * BN * 4 + 4 * BN * 4;
-  static constexpr int kStagesRaw = WS ? (227 * 1024 - kFixed - (int)kWBytes) / (int)kStageBytes : (180 * 1024) / (int)kStageBytes;
+  static constexpr int kFixed = 1024 + 256 + (2 * pnx::kEpiWarps + 5) * BN * 4;
+  static constexpr int kStagesRaw = (227 * 1024 - kFixed - (int)kWBytes) / (int)kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
   static constexpr size_t kSmem = kFixed + kWBytes + (size_t)kStages * kStageBytes;
   static_assert(kStages >= 2, "stages");
@@ -73,13 +56,13 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       : "memory");
 }
 
-__device__ __forceinline__ uint64_t desc_sw128_off(uint32_t addr, uint32_t sbo, uint32_t base_off) {
-  return pnx::make_smem_desc_sw128(addr, 0, sbo) | ((uint64_t)(base_off & 7u) << 49);
+__device__ __forceinline__ uint64_t desc_sw128_off(uint32_t addr, uint32_t base_off) {
+  return pnx::make_smem_desc_sw128(addr, 16, 1024) | ((uint64_t)(base_off & 7u) << 49);
 }
 
-template <int BN, bool WS>
-__global__ void __launch_bounds__(320, 1) igemm_win_kernel(const __grid_constant__ CUtensorMap amap,
-                                                           const __grid_constant__ CUtensorMap wmap, WinParams p) {
+template <int BN, bool WS, int F>
+__global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_constant__ CUtensorMap amap,
+                                                                const __grid_constant__ CUtensorMap wmap, WinParams p) {
   using C = WCfgWin<BN, WS>;
   constexpr int kStages = C::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -87,50 +70,39 @@ __global__ void __launch_bounds__(320, 1) igemm_win_kernel(const __grid_constant
   uint8_t* smem = smem_w + C::kWBytes;  // stage ring (the stationary weight tiles, if any, come first)
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)kStages * C::kStageBytes);
   uint64_t* empty = full + kStages;
-  uint64_t* tfull = empty + kStages;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* wfull = tempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
-  uint8_t* s_slab = reinterpret_cast<uint8_t*>(full) + 256;
-  float* s_stat = reinterpret_cast<float*>(s_slab + 8 * 4096);
-  float* s_bias = s_stat + 2 * BN;
+  uint64_t* wfull = empty + kStages;
+  float* s_stat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);  // [8 warps][2][BN] per-channel sums
+  float* s_bias = s_stat + pnx::kEpiWarps * 2 * BN;
   float* s_bnc = s_bias + BN;   // [4][BN] fused BN-backward: scale, shift, mean, invstd of this CTA's columns
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && pnx::elect_one()) {
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  const int n0 = blockIdx.y * BN;
+  if (threadIdx.x == 0) {
     pnx::tma_prefetch_desc(&amap);
     pnx::tma_prefetch_desc(&wmap);
     for (int s = 0; s < kStages; ++s) {
       pnx::mbar_init(&full[s], 1);
-      pnx::mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      pnx::mbar_init(&tfull[a], 1);
-      pnx::mbar_init(&tempty[a], 8);
+      pnx::mbar_init(&empty[s], 8);  // one arrival per consumer warp
     }
     pnx::mbar_init(wfull, 1);
     pnx::fence_barrier_init();
   }
-  if (warp == 1) pnx::tmem_alloc<512>(tmem_slot);
   if (p.bias)
-    for (int c = threadIdx.x; c < BN; c += blockDim.x) s_bias[c] = p.bias[blockIdx.y * BN + c];
-  for (int c = threadIdx.x; c < 2 * BN; c += blockDim.x) s_stat[c] = 0.f;
-  if (p.bnr_raw)
+    for (int c = threadIdx.x; c < BN; c += blockDim.x) s_bias[c] = p.bias[n0 + c];
+  for (int c = threadIdx.x; c < pnx::kEpiWarps * 2 * BN; c += blockDim.x) s_stat[c] = 0.f;
+  if (F == 1)
     for (int c = threadIdx.x; c < BN; c += blockDim.x) {
-      const int gc = blockIdx.y * BN + c;
+      const int gc = n0 + c;
       s_bnc[c] = p.bnr_scale[gc]; s_bnc[BN + c] = p.bnr_shift[gc]; s_bnc[2 * BN + c] = p.bnr_mean[gc]; s_bnc[3 * BN + c] = p.bnr_invstd[gc];
     }
-  pnx::tc_fence_before();
   __syncthreads();
-  pnx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int num_tiles = p.B * p.H * p.XC;
-  const int n0 = blockIdx.y * BN;
   const int kcc = p.Cin >> 6;
 
-  if (warp == 0) {
-    if (pnx::elect_one()) {
+  if (wg == 0) {
+    pnx::regs_dealloc<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       if (WS) {
@@ -154,217 +126,73 @@ __global__ void __launch_bounds__(320, 1) igemm_win_kernel(const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (pnx::elect_one()) {
-      constexpr uint32_t idesc = pnx::make_idesc_bf16(128, BN, 0, 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      if (WS) pnx::mbar_wait(wfull, 0);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        pnx::mbar_wait(&tempty[acc], acc_phase ^ 1);
-        pnx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        bool first = true;
-        for (int kc = 0; kc < kcc * 3; ++kc) {
-          pnx::mbar_wait(&full[stage], phase);
-          pnx::tc_fence_after();
-          const uint32_t a_base = pnx::smem_u32(smem + (size_t)stage * C::kStageBytes);
-          // WS: kcc == 1, so stage kc is kernel row r = kc and its taps are weight tiles 3r .. 3r+2
-          const uint32_t b_base = WS ? pnx::smem_u32(smem_w) + kc * 3 * C::kBTap : a_base + kWinSlot;
-#pragma unroll
-          for (int s = 0; s < 3; ++s) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t da = desc_sw128_off(a_base + s * 128 + k * 32, 1024, p.base_off_mode ? (uint32_t)s : 0u);
-              const uint64_t db = pnx::make_smem_desc_sw128(b_base + s * C::kBTap + k * 32, 0, 1024);
-              pnx::umma_f16(d_tmem, da, db, idesc, first ? 0u : 1u);
-              first = false;
-            }
-          }
-          pnx::umma_commit(&empty[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        pnx::umma_commit(&tfull[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
   } else {
-    // ---------------------------------------------------------------- epilogue
-    // 8 warps: two per TMEM lane quarter; the 64-column block pairs of a tile alternate between the two groups (and
-    // the alternation flips every tile, so odd pair counts balance over the two accumulator sets)
-    const int quarter = warp & 3, group = (warp - 2) >> 2;
-    int acc = 0, ti = 0;
-    uint32_t acc_phase = 0;
-    uint8_t* slab = s_slab + (warp - 2) * 4096;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++ti) {
+    pnx::regs_alloc<224>();
+    const int half = wg - 1;  // pixels [64 * half, 64 * half + 64) of every tile
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    if (WS) pnx::mbar_wait(wfull, 0);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int xc = tile % p.XC, by = tile / p.XC;
-      const long long row0 = (long long)by * p.W + xc * 128;          // pixel index of tile row 0 (by = b*H + y)
-      const int valid = min(128, p.W - xc * 128);                       // pixels of this image row in the tile
-      while (!pnx::mbar_try_wait(&tfull[acc], acc_phase)) __nanosleep(64);
-      pnx::tc_fence_after();
-      const int nrows = max(0, min(32, valid - quarter * 32));
-#pragma unroll 1
-      for (int cb = 0; cb < BN / 32; ++cb) {
-        if ((((cb >> 1) + ti) & 1) != group) continue;
-        uint32_t r[32];
-        pnx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BN + cb * 32, r);
-        pnx::tmem_ld_wait();
-        float v[32];
+      int prev = 0;
+      for (int kc = 0; kc < kcc * 3; ++kc) {
+        pnx::mbar_wait(&full[stage], phase);
+        pnx::wgmma_fence();
+        pnx::fence_acc(acc);
+        const uint32_t a_base = pnx::smem_u32(smem + (size_t)stage * C::kStageBytes) + half * 64 * 128;
+        // WS: kcc == 1, so stage kc is kernel row r = kc and its taps are weight tiles 3r .. 3r+2
+        const uint32_t b_base = WS ? pnx::smem_u32(smem_w) + kc * 3 * C::kBTap : pnx::smem_u32(smem + (size_t)stage * C::kStageBytes) + kWinSlot;
 #pragma unroll
-        for (int k = 0; k < 32; ++k) v[k] = __uint_as_float(r[k]);
-        if (p.bias) {
+        for (int s = 0; s < 3; ++s) {
 #pragma unroll
-          for (int k = 0; k < 32; k += 4) {
-            const float4 bq = *reinterpret_cast<const float4*>(s_bias + cb * 32 + k);
-            v[k] += bq.x; v[k + 1] += bq.y; v[k + 2] += bq.z; v[k + 3] += bq.w;
+          for (int k = 0; k < 4; ++k) {
+            const uint64_t da = desc_sw128_off(a_base + s * 128 + k * 32, p.base_off_mode ? (uint32_t)s : 0u);
+            const uint64_t db = pnx::make_smem_desc_sw128(b_base + s * C::kBTap + k * 32, 16, 1024);
+            pnx::Wgmma<BN, 0, 0>::mma(acc, da, db, (kc > 0 || s > 0 || k > 0) ? 1u : 0u);
           }
         }
-        if (p.relu) {
-#pragma unroll
-          for (int k = 0; k < 32; ++k) v[k] = fmaxf(v[k], 0.f);
-        }
-        const int half = cb & 1;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint4 pk = make_uint4(pnx::pack_bf16x2(v[8 * k], v[8 * k + 1]), pnx::pack_bf16x2(v[8 * k + 2], v[8 * k + 3]),
-                                      pnx::pack_bf16x2(v[8 * k + 4], v[8 * k + 5]), pnx::pack_bf16x2(v[8 * k + 6], v[8 * k + 7]));
-          *reinterpret_cast<uint4*>(slab + lane * 128 + (((half * 4 + k) ^ (lane & 7)) << 4)) = pk;
-        }
-        if (half == 1) {
-          __syncwarp();
-          const int ch = lane & 7;
-          if (p.bnr_raw) {
-            // fused BatchNorm-backward reduce (igemm.cu): gate from raw, store g = dy * gate, accumulate sum g / sum g*xhat
-            const int c8 = (cb - 1) * 32 + ch * 8;
-            float sg[8], sgx[8], csc[8], csh[8], cmu[8], cis[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              sg[k] = sgx[k] = 0.f;
-              csc[k] = s_bnc[c8 + k]; csh[k] = s_bnc[BN + c8 + k]; cmu[k] = s_bnc[2 * BN + c8 + k]; cis[k] = s_bnc[3 * BN + c8 + k];
-            }
-            uint4 rws[8];
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int row = it * 4 + (lane >> 3);
-              rws[it] = make_uint4(0u, 0u, 0u, 0u);
-              if (row < nrows) rws[it] = __ldg(reinterpret_cast<const uint4*>(p.bnr_raw + (row0 + quarter * 32 + row) * p.bnr_ld + n0 + c8));
-            }
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int row = it * 4 + (lane >> 3);
-              if (row < nrows) {
-                float d[8], rw[8];
-                unpack_bf16x8(*reinterpret_cast<const uint4*>(slab + row * 128 + ((ch ^ (row & 7)) << 4)), d);
-                unpack_bf16x8(rws[it], rw);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                  const float g = fmaf(rw[k], csc[k], csh[k]) > 0.f ? d[k] : 0.f;
-                  d[k] = g;
-                  sg[k] += g;
-                  sgx[k] = fmaf(g, (rw[k] - cmu[k]) * cis[k], sgx[k]);
-                }
-                *reinterpret_cast<uint4*>(p.out + (row0 + quarter * 32 + row) * p.ldc + n0 + (cb - 1) * 32 + ch * 8) =
-                    make_uint4(pnx::pack_bf16x2(d[0], d[1]), pnx::pack_bf16x2(d[2], d[3]), pnx::pack_bf16x2(d[4], d[5]), pnx::pack_bf16x2(d[6], d[7]));
-              }
-            }
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              sg[k] += __shfl_xor_sync(0xffffffffu, sg[k], 8);
-              sgx[k] += __shfl_xor_sync(0xffffffffu, sgx[k], 8);
-              sg[k] += __shfl_xor_sync(0xffffffffu, sg[k], 16);
-              sgx[k] += __shfl_xor_sync(0xffffffffu, sgx[k], 16);
-            }
-            if (lane < 8) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                atomicAdd(&s_stat[c8 + k], sg[k]);
-                atomicAdd(&s_stat[BN + c8 + k], sgx[k]);
-              }
-            }
-          } else {
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int row = it * 4 + (lane >> 3);
-            if (row < nrows) {
-              const uint4 val = *reinterpret_cast<const uint4*>(slab + row * 128 + ((ch ^ (row & 7)) << 4));
-              *reinterpret_cast<uint4*>(p.out + (row0 + quarter * 32 + row) * p.ldc + n0 + (cb - 1) * 32 + ch * 8) = val;
-            }
-          }
-          }
-          if (p.stats) {
-            float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-            const int cpc = lane >> 2, cps = (lane & 3) * 4;
-              // full 32-row blocks (all but the ragged tile edge): unrolled so the 32 LDS are in flight together
-              if (nrows == 32) {
-#pragma unroll
-                for (int row = 0; row < 32; ++row) {
-                  const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(slab + row * 128 + ((cpc ^ (row & 7)) << 4) + cps);
-                  const float2 f = __bfloat1622float2(h2);
-                  s0 += f.x; s1 += f.y;
-                  q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-                }
-              } else {
-                for (int row = 0; row < nrows; ++row) {
-                  const __nv_bfloat162 h2 = *reinterpret_cast<const __nv_bfloat162*>(slab + row * 128 + ((cpc ^ (row & 7)) << 4) + cps);
-                  const float2 f = __bfloat1622float2(h2);
-                  s0 += f.x; s1 += f.y;
-                  q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-                }
-              }
-            const int c0 = (cb - 1) * 32 + 2 * lane;
-            if (p.stats_direct) {   // deterministic mode: order-insensitive fp64 accumulation (pnx_set_deterministic)
-              atomicAdd(&p.stats[n0 + c0], (double)s0); atomicAdd(&p.stats[n0 + c0 + 1], (double)s1);
-              atomicAdd(&p.stats[p.stats_C + n0 + c0], (double)q0); atomicAdd(&p.stats[p.stats_C + n0 + c0 + 1], (double)q1);
-            } else {
-              atomicAdd(&s_stat[c0], s0); atomicAdd(&s_stat[c0 + 1], s1);
-              atomicAdd(&s_stat[BN + c0], q0); atomicAdd(&s_stat[BN + c0 + 1], q1);
-            }
-          }
-          __syncwarp();
-        }
+        pnx::wgmma_commit();
+        pnx::wgmma_wait<1>();
+        if (kc > 0 && lane == 0) pnx::mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
-      pnx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) pnx::mbar_arrive(&tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
+      pnx::wgmma_wait<0>();
+      pnx::fence_acc(acc);
+      if (lane == 0) pnx::mbar_arrive(&empty[prev]);
+      const long long row0 = (long long)by * p.W + xc * 128;  // pixel index of tile row 0 (by = b*H + y)
+      pnx::gemm_epilogue<BN, F>(acc, p.epi, row0, min(128, p.W - xc * 128), half, n0, s_bias, s_stat, s_bnc);
     }
-    if (p.stats && !p.stats_direct) {
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-      for (int c = threadIdx.x - 64; c < BN; c += 256) {
-        atomicAdd(&p.stats[n0 + c], (double)s_stat[c]);
-        atomicAdd(&p.stats[p.stats_C + n0 + c], (double)s_stat[BN + c]);
-      }
-    } else if (p.bnr_raw) {
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-      for (int c = threadIdx.x - 64; c < BN; c += 256) {
-        atomicAdd(&p.bnr_red[n0 + c], (double)s_stat[c]);
-        atomicAdd(&p.bnr_red[p.bnr_C + n0 + c], (double)s_stat[BN + c]);
-      }
-    }
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+    pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, threadIdx.x - 128, 256);
   }
-  pnx::tc_fence_before();
-  __syncthreads();
-  pnx::tc_fence_after();
-  if (warp == 1) pnx::tmem_dealloc<512>(tmem_base);
 }
 
-template <int BN, bool WS>
-int launch_win(const CUtensorMap& amap, const CUtensorMap& wmap, const WinParams& p, int n_blocks, int sm_count,
-               cudaStream_t stream) {
+template <int BN, bool WS, int F>
+int launch_win_f(const CUtensorMap& amap, const CUtensorMap& wmap, const WinParams& p, int n_blocks, int sm_count,
+                 cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    PNX_CUDA(cudaFuncSetAttribute(igemm_win_kernel<BN, WS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WCfgWin<BN, WS>::kSmem));
+    PNX_CUDA(cudaFuncSetAttribute(igemm_win_kernel<BN, WS, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WCfgWin<BN, WS>::kSmem));
     attr_set = true;
   }
   const int num_tiles = p.B * p.H * p.XC;
   int gx = sm_count / n_blocks;
   if (gx < 1) gx = 1;
   if (gx > num_tiles) gx = num_tiles;
-  igemm_win_kernel<BN, WS><<<dim3(gx, n_blocks), 320, WCfgWin<BN, WS>::kSmem, stream>>>(amap, wmap, p);
+  igemm_win_kernel<BN, WS, F><<<dim3(gx, n_blocks), kThreads, WCfgWin<BN, WS>::kSmem, stream>>>(amap, wmap, p);
   PNX_CHECK_LAUNCH();
   return PNX_OK;
+}
+
+template <int BN, bool WS>
+int launch_win(const CUtensorMap& amap, const CUtensorMap& wmap, const WinParams& p, int n_blocks, int sm_count,
+               cudaStream_t stream) {
+  if (p.epi.bnr_raw) return launch_win_f<BN, WS, 1>(amap, wmap, p, n_blocks, sm_count, stream);
+  return launch_win_f<BN, WS, 0>(amap, wmap, p, n_blocks, sm_count, stream);
 }
 
 }  // namespace
@@ -382,14 +210,19 @@ extern "C" int pnx_conv3x3_win(const void* A, long long lda, int B, int H, int W
   PNX_CHECK_ARG(Cin % 64 == 0 && Cout % block_n == 0, "Cin % 64, Cout % block_n");
   PNX_CHECK_ARG(lda % 8 == 0 && ldc % 8 == 0, "lda/ldc % 8");
   PNX_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "alignment");
-  if (sm_count <= 0) sm_count = 148;
+  if (sm_count <= 0) sm_count = 132;
   WinParams p;
   p.B = B; p.H = H; p.W = W; p.XC = (W + 127) / 128;
   p.Cin = Cin; p.Cout_total = Cout;
-  p.out = (__nv_bfloat16*)out; p.ldc = ldc; p.bias = bias; p.stats = stats; p.stats_C = stats_C; p.relu = relu;
-  p.stats_direct = g_pnx_deterministic;
+  p.bias = bias;
   p.base_off_mode = base_off_mode;
-  p.bnr_raw = (const __nv_bfloat16*)bnr_raw; p.bnr_ld = bnr_ld; p.bnr_scale = bnr_scale; p.bnr_shift = bnr_shift;
+  pnx::EpiParams& e = p.epi;
+  e.out = out; e.ldc = ldc; e.has_bias = bias != nullptr; e.relu = relu;
+  e.addend = nullptr; e.addend_f32 = nullptr; e.ld_add = 0;
+  e.stats = stats; e.stats_C = stats_C; e.stats_mod = 1 << 30; e.stats_direct = g_pnx_deterministic;
+  e.shuffle = 0; e.Hout = H; e.Wout = W;
+  e.bnr_raw = (const __nv_bfloat16*)bnr_raw; e.bnr_ld = bnr_ld;
+  p.bnr_scale = bnr_scale; p.bnr_shift = bnr_shift;
   p.bnr_mean = bnr_mean; p.bnr_invstd = bnr_invstd; p.bnr_red = bnr_red; p.bnr_C = bnr_C;
   if (bnr_raw)
     PNX_CHECK_ARG(!stats && bnr_scale && bnr_shift && bnr_mean && bnr_invstd && bnr_red && bnr_C == Cout && bnr_ld % 8 == 0 &&

@@ -1,4 +1,4 @@
-// pfn.cu -- PillarFeatureNet encoder (rows V3, P1-P3 of SURVEY.md section 8a) for sm_100a, fp32.
+// pfn.cu -- PillarFeatureNet encoder (rows V3, P1-P3 of SURVEY.md section 8a) for sm_90a, fp32.
 //
 // Replaces reference det3d/models/readers/pillar_encoder.py:113-123 (scatter_mean + decoration),
 // :35-50 (PFNLayer: Linear(no bias) -> BatchNorm1d(eps 1e-3) -> ReLU -> scatter_max -> gather -> cat)

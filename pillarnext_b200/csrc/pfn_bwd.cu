@@ -1,4 +1,4 @@
-// pfn_bwd.cu -- backward of the PillarFeatureNet encoder (rows P1-P3), fp32, sm_100a.
+// pfn_bwd.cu -- backward of the PillarFeatureNet encoder (rows P1-P3), fp32, sm_90a.
 // The reference gets this from autograd through torch_scatter.scatter_max / BatchNorm1d / Linear
 // (det3d/models/readers/pillar_encoder.py:35-50,174-182; trainer/trainer/trainer.py:94-108).
 // Same bucketed layout as the forward (pfn.cu): per-pillar work is an in-order loop, no atomics on any

@@ -1,13 +1,15 @@
-// pnx_common.cuh -- shared device helpers for the pillarnext_b200 sm_100a kernels.
-// Raw PTX wrappers for mbarrier / TMA (cp.async.bulk.tensor) / tcgen05 (UMMA + TMEM) / cp.async.
-// Descriptor bit layouts follow the PTX ISA "tcgen05 shared memory descriptor" and
-// "instruction descriptor" tables (cross-checked against CUTLASS cute/arch/mma_sm100_desc.hpp).
+// pnx_common.cuh -- shared device helpers for the pillarnext_b200 sm_90a kernels.
+// Raw PTX wrappers for mbarrier / TMA (cp.async.bulk.tensor) / cp.async / wgmma.
+// The wgmma shared-memory descriptor layout follows the PTX ISA "matrix descriptor" table
+// (cross-checked against CUTLASS cute/arch/mma_sm90_desc.hpp).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma_sm90.cuh"
 
 #define PNX_OK 0
 #define PNX_ERR_ARG -1
@@ -109,96 +111,52 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       : "memory");
 }
 
-// tile::gather4: four arbitrary rows (r0..r3) of a 2-D tensor, box = [box_cols x 1]; the rows land consecutively at
-// dst (128B swizzle by absolute smem address); a row index outside [0, rows) is zero-filled and still counted in
-// the mbarrier transaction bytes (measured: tools/gather4_rate.cu).
-__device__ __forceinline__ void tma_gather4(const CUtensorMap* m, uint64_t* bar, uint32_t dst, int c0, int r0, int r1,
-                                            int r2, int r3) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6, %7}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-      : "memory");
+// ------------------------------------------------------------------ cp.async (gathered rows)
+// 16-byte global -> shared copy; src_bytes = 0 zero-fills the destination (absent neighbour / padding row)
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+// arrive on `bar` once every cp.async this thread issued so far has landed (counts as one of the barrier's arrivals)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// offset of 16-byte chunk `chunk` of row `row` in a 128B-swizzled tile (TMA SWIZZLE_128B / wgmma SW128 layout)
+__device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
+  return row * 128u + ((chunk ^ (row & 7u)) << 4);
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// tcgen05.commit: arrive on an mbarrier when all previously issued MMAs of this thread complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// ------------------------------------------------------------------ wgmma (sm_90a)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins accumulator registers in place around the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16/f16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+// producer warpgroup hands registers to the accumulator-holding warpgroups
+template <uint32_t kRegs>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 
-// Instruction descriptor for kind::f16: D=f32, A=B=bf16.
-//  [4,6) D fmt (1=f32) | [7,10) A fmt (1=bf16) | [10,13) B fmt | 15 A major (0=K,1=MN) | 16 B major
-//  [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, SWIZZLE_128B.
-//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2 = SW128)
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+// wgmma shared-memory descriptor, SWIZZLE_128B: [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset |
+// [62,64) layout (1 = SW128).  SBO = stride of 8-row groups; MN-major: LBO = stride of 64-element MN atoms.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-// TMEM -> registers: 32 lanes x 32 columns of 32-bit (each thread: its lane's 32 consecutive columns)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// row / column of accumulator register i of this thread in its warpgroup's 64 x N wgmma tile
+__device__ __forceinline__ int acc_row(int i) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int acc_col(int i) { return 8 * (i >> 2) + 2 * (threadIdx.x & 3) + (i & 1); }
 
 // ------------------------------------------------------------------ misc
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -211,7 +169,5 @@ __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(_
 
 // host: encode a 2-D bf16 tensor map (rows x cols, row-major), box = box_rows x box_cols, SWIZZLE_128B.
 // Resolved through cudaGetDriverEntryPoint so the library links without libcuda.
-int pnx_encode_tmap_gather_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                                uint64_t row_stride_bytes);
 int pnx_encode_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                             uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols);

@@ -1,4 +1,4 @@
-// postproc.cu -- detection decode + rotated NMS of the CenterPoint head (row F1 of SURVEY.md section 8f), sm_100a.
+// postproc.cu -- detection decode + rotated NMS of the CenterPoint head (row F1 of SURVEY.md section 8f), sm_90a.
 //
 // Replaces CenterHead.predict / post_processing (reference det3d/models/heads/centerhead.py:231-384),
 // rotate_nms_pcdet (det3d/core/bbox/box_torch_ops.py:5-31) and the native NMS it calls

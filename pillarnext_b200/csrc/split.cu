@@ -3,7 +3,7 @@
 // The reference computes the whole path in fp32 (no autocast anywhere: det3d/models/necks/aspp.py:19-32,
 // heads/centerhead.py:128-136, utils/sparse_conv.py:31-39).  The production path stores activations as bf16; this
 // mode stores every activation row as a PAIR of bf16 values (hi = bf16(v), lo = bf16(v - hi), ~16 mantissa bits,
-// hi at column c and lo at column lo_off + c of the same row matrix) and runs the same tcgen05 kernels over the
+// hi at column c and lo at column lo_off + c of the same row matrix) and runs the same wgmma kernels over the
 // hi/lo segments (igemm.cu nseg, three wgrad launches), with raw convolution outputs, BatchNorm arithmetic and
 // gradient accumulation in fp32.  It exists to show that the kernels reproduce the reference's numbers to the
 // north-star tolerance (1e-3 abs on heat-maps / boxes); the kernels here are the row-wise glue of that mode:

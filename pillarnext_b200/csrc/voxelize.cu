@@ -1,4 +1,4 @@
-// voxelize.cu -- dynamic point->pillar voxelizer (rows V1-V3 of SURVEY.md section 8a) for sm_100a.
+// voxelize.cu -- dynamic point->pillar voxelizer (rows V1-V3 of SURVEY.md section 8a) for sm_90a.
 //
 // Replaces, bit-exactly on the indices, reference det3d/models/readers/pillar_encoder.py:86-125:
 //   (xyz-min)/voxel (fp32 sub + IEEE fp32 divide), float-domain range test on x,y only, trunc,

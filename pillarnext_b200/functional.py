@@ -14,7 +14,7 @@ from . import ops
 # ------------------------------------------------------------------------------------------- precision mode
 # "bf16"  : production path -- bf16 tensor-core operands and stored activations, fp32 accumulation.
 # "split" : fp32-grade parity mode -- every activation is a (hi, lo) bf16 pair ([M, 2C] rows, include/pnx.h "split
-#           rows"), the same tcgen05 kernels run over the hi/lo segments, raw conv outputs / BatchNorm / gradient sums
+#           rows"), the same wgmma kernels run over the hi/lo segments, raw conv outputs / BatchNorm / gradient sums
 #           are fp32.  ~3x the tensor work and ~3x the bytes: used to demonstrate the north-star tolerance (1e-3 abs
 #           vs the fp32 reference), not for throughput.
 _PRECISION = "bf16"
@@ -57,7 +57,6 @@ def set_deterministic(on):
     """Opt-in reproducible reductions for the bf16 path (debugging / regression hunting; slower):
       * BatchNorm statistics of the conv epilogues accumulate in fp64 (order effects 1e-16 instead of 1e-7), the fused
         BatchNorm-backward reduce is switched off in favour of the separate pass (fixed order inside a CTA, fp64 across CTAs);
-      * weight gradients: every K split writes its own slab, the slabs are added in split order (no fp32 atomics).
     With it two runs of the same step give a bit-identical forward and bit-identical parameter gradients
     (tests/test_precision_gpu.py::test_run_to_run_spread_of_the_gradients; "bit-identical" up to the 1e-16 order effects
     of the remaining fp64 atomics, which vanish in the rounding to fp32).  Not covered: three or more positives of one
@@ -279,11 +278,10 @@ class BNInfo:
         self.fused = False
 
 
-# The fused reduce adds ~7 instructions per output element to the GEMM epilogue.  Measured on the B200 (round 2): for the
-# 3x3 convolutions (K = 9 * C >= 576 MMA steps per tile) it hides under the MMA loop (+4 % on the head's 384 -> 64 data
-# gradient) and removes a full sweep over dy and raw; for the thin GEMMs (the head's final-conv data gradient, K = 192,
-# and the ConvTranspose2d one, K = 256) the epilogue is already the bottleneck and the fusion costs more than the
-# separate pass (0.99 -> 3.6 ms per step) -- so it is applied only above this K.
+# The fused reduce adds ~7 instructions per output element to the GEMM epilogue.  For the 3x3 convolutions (K = 9 * C >=
+# 576 MMA steps per tile) that is small against the MMA loop and it removes a full sweep over dy and raw; for the thin
+# GEMMs (the head's final-conv data gradient, K = 192, and the ConvTranspose2d one, K = 256) the epilogue is already the
+# larger part of the kernel -- so it is applied only above this K.
 FUSE_BN_REDUCE_MIN_K = 512
 
 

@@ -2,7 +2,7 @@
 
 Same class names, constructor kwargs, forward signatures and state-dict keys as the reference
 (SURVEY.md section 8b) so hydra's `_target_` strings, `load_checkpoint(strict=True)`, DDP and
-`tools/train.py` / `tools/test.py` work unchanged -- but every forward/backward runs in libpnx (sm_100a).
+`tools/train.py` / `tools/test.py` work unchanged -- but every forward/backward runs in libpnx (sm_90a).
 The drop-in module paths live in the top-level `det3d/` package, which re-exports these classes.
 
   PillarFeatureNet  <- det3d/models/readers/pillar_encoder.py:128-182
@@ -25,7 +25,7 @@ from . import ops
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise RuntimeError("pillarnext_b200.%s runs on CUDA (sm_100a) only -- there is no CPU path" % what)
+        raise RuntimeError("pillarnext_b200.%s runs on CUDA (sm_90a) only -- there is no CPU path" % what)
 
 
 # =========================================================================================== reader
@@ -352,7 +352,7 @@ class ASPPNeck(nn.Module):
         self.in_channels = in_channels
 
     def forward(self, x):
-        """aspp.py:19-40 (activation checkpointing dropped: values identical, B200 has the memory)."""
+        """aspp.py:19-40 (activation checkpointing dropped: values identical, the 80 GB of an H100 hold the activations)."""
         _require_cuda(x, "ASPPNeck")
         rows, B, H, W = _to_rows(x)
         C = self.in_channels

@@ -115,10 +115,9 @@ class Voxels:
                                "by ascending batch index; use voxelize(..., frame_sorted=False)" % bad)
 
 
-# The frame-tiled kernels (pnx_voxelize_frames) are bit-exact but, measured on the B200, NOT faster than the global-bitmap
-# ones at any batch size (256 nuScenes frames: 416 us vs 290 us; ncu: instruction-issue bound, 139 M + 96 M warp
-# instructions -- every slice re-processes all points of its frame and the bitmap sweeps cost as much as the points), so
-# they only run on request (frame_sorted="force"); None = never chosen automatically.
+# The frame-tiled kernels (pnx_voxelize_frames) are bit-exact with the global-bitmap ones, but every slice re-processes all
+# points of its frame and its bitmap sweep costs as much as the points, so they only run on request
+# (frame_sorted="force"; bench.py reports their time next to the production kernels); None = never chosen automatically.
 FRAME_TILED_MIN_CTAS = None
 
 
@@ -472,7 +471,7 @@ def igemm(A, M, w_packed, taps, cin, cout, out, *, lda=None, ldc=None, nbr=None,
     return out
 
 
-WIN_BASE_OFF = 0   # measured on B200: the 128B swizzle is applied on absolute smem address bits, so row-shifted
+WIN_BASE_OFF = 0   # measured on H100: the 128B swizzle is applied on absolute smem address bits, so row-shifted wgmma
                    # descriptors need NO matrix base offset (tests/test_igemm_win_gpu.py checks both conventions)
 
 
@@ -512,8 +511,8 @@ DETERMINISTIC = False     # set through functional.set_deterministic
 
 
 def set_deterministic(on):
-    """Library side of functional.set_deterministic: ordered split-K reduction in pnx_wgrad (per-split slabs added in split
-    order) and fp64 accumulation of the BatchNorm statistics in the GEMM epilogues (pnx_set_deterministic)."""
+    """Library side of functional.set_deterministic: fp64 accumulation of the BatchNorm statistics in the GEMM epilogues
+    (pnx_set_deterministic).  pnx_wgrad reduces its K splits in split order in either mode."""
     global DETERMINISTIC
     prev, DETERMINISTIC = DETERMINISTIC, bool(on)
     lib().pnx_set_deterministic(1 if on else 0)
@@ -537,11 +536,10 @@ def wgrad(X, x_channels, Y, y_channels, M, taps, dW, *, nbr=None, dense=None, sh
     d = dense or (0, 0, 0, 0, 1, 1, 1, 0)
     if gathered is None:
         gathered = nbr is not None or dense is not None or shuffle
-    partials = None
-    if DETERMINISTIC and M > 0:
-        splits = lib().pnx_wgrad_splits(x_channels, y_channels, taps, M, sm_count())
-        partials = torch.empty(splits * taps * x_channels * y_channels, dtype=torch.float32, device=dW.device)
-    _count(2 if partials is not None else 1)
+    # one slab per K split, added in split order (not fp32 atomics): the weight gradient is the same from run to run
+    splits = lib().pnx_wgrad_splits(x_channels, y_channels, taps, M, sm_count())
+    partials = torch.empty(max(splits, 1) * taps * x_channels * y_channels, dtype=torch.float32, device=dW.device)
+    _count(2)
     with _Timed("wgrad", 2.0 * M * taps * x_channels * y_channels, 2.0 * M * (x_channels + taps * y_channels),
                 "M%d_T%d_X%d_Y%d" % (M, taps, x_channels, y_channels)):
       check(lib().pnx_wgrad(ptr(X), X.stride(0), x_channels, ptr(Y), Y.stride(0), Y.shape[0], y_channels, 1 if gathered else 0, M,
@@ -702,7 +700,7 @@ def relu_bwd_split(dy_f32, y, y_lo, M, C, g, g_lo):
 
 def wgrad_split(X, x_lo, x_channels, Y, y_lo, y_channels, M, taps, dW, **kw):
     """Weight gradient of split operands: one launch per (X piece, Y piece) segment, smallest products first, all
-    accumulating (fp32 red.global.add) into the same dW."""
+    accumulating into the same dW."""
     for xp, yp in split_segments():
         wgrad(X[:, xp * x_lo:xp * x_lo + x_channels], x_channels, Y[:, yp * y_lo:yp * y_lo + y_channels], y_channels, M, taps, dW, **kw)
     return dW

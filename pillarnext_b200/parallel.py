@@ -2,7 +2,7 @@
 the sampler, gradients averaged over the ranks (reference: torch DDP with 25 MB buckets overlapped with the backward,
 tools/train.py:53-62).  BatchNorm statistics are local unless modules.enable_sync_batchnorm() is used.
 
-BucketedGradAllReduce is the B200 version of the DDP reducer for this model: the parameters are grouped into a few
+BucketedGradAllReduce is this package's version of the DDP reducer for this model: the parameters are grouped into a few
 buckets in backward order (head, neck, backbone + reader); a bucket is reduced as soon as the last of its gradients has
 been accumulated -- one fused `cat` into a flat fp32 buffer, one NCCL all-reduce (NVLink/NVSwitch) and one fused copy
 back, all on a side stream -- while the backward of the earlier layers is still running on the main stream.  Per step

@@ -2,7 +2,7 @@
 package's entry points (row F4): fit / train_epoch / val_epoch, AdamW step with gradient clipping (35) and a
 per-iteration OneCycleLR step, checkpoints in the reference's format ({"meta", "state_dict", "optimizer", "scheduler"},
 trainer/utils/checkpoint.py:62-89, `module.` prefix stripped on load), detections gathered over the ranks and handed to
-`dataset.evaluation`.  Differences that are the point of the B200 path: inputs move with non-blocking copies, the
+`dataset.evaluation`.  Differences that are the point of the GPU path: inputs move with non-blocking copies, the
 gradient all-reduce is the bucketed / overlapped reducer of parallel.py instead of DDP, losses are logged from device
 values read once per logging interval (the reference's `.cpu()` log values synchronise every iteration)."""
 import logging

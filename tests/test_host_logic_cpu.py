@@ -15,6 +15,9 @@ def test_wgrad_splits_channel_counts_the_kernel_does_not_tile(monkeypatch):
             calls.append(dict(x_off=X, ldx=ldx, xc=xc, yc=yc, taps=taps, dW=dW_ptr))
             return 0
 
+        def pnx_wgrad_splits(self, xc, yc, taps, M, sm_count):
+            return 2
+
     monkeypatch.setattr(ops, "lib", lambda: FakeLib())
     monkeypatch.setattr(ops, "ptr", lambda t: None if t is None else t.data_ptr())
     monkeypatch.setattr(ops, "stream", lambda: 0)

@@ -1,4 +1,4 @@
-"""tcgen05 gather implicit-GEMM vs a plain torch fp32 reference on the SAME bf16-rounded operands
+"""wgmma gather implicit-GEMM vs a plain torch fp32 reference on the SAME bf16-rounded operands
 (fp32 accumulate): tolerance 2e-3 relative to the output scale (accumulation order only) plus the
 final bf16 rounding (2^-8 relative) when the output is bf16."""
 import pytest

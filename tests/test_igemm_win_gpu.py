@@ -1,4 +1,4 @@
-"""TMA-window 3x3 convolution (pnx_conv3x3_win: im2col folded into 4-D TMA loads, horizontally shifted UMMA
+"""TMA-window 3x3 convolution (pnx_conv3x3_win: im2col folded into 4-D TMA loads, horizontally shifted wgmma
 descriptors) vs torch fp32 conv2d on the same bf16 operands (tolerance: accumulation order + bf16 output rounding)."""
 import pytest
 import torch
@@ -31,7 +31,7 @@ def run(B, H, W, Cin, Cout, bn, base_off, bias=True, relu=True):
 
 
 def test_descriptor_base_offset_convention():
-    """Exactly one UMMA base-offset convention reproduces the shifted windows; it must be the library default."""
+    """Exactly one wgmma descriptor base-offset convention reproduces the shifted windows; it must be the library default."""
     e1, _ = run(1, 6, 200, 64, 64, 64, 1)
     e0, _ = run(1, 6, 200, 64, 64, 64, 0)
     print("rel err with base_offset=(start>>7)&7: %.3g ; with base_offset=0: %.3g" % (e1, e0))

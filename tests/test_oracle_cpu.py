@@ -1,6 +1,5 @@
-"""CPU tier: pins the oracle restatement against (a) the golden vectors frozen from the reference's own
-files (tests/golden/ref_tiny.npz, made by oracle/make_golden.py) and (b) the reference itself when
-/root/reference is present; checks the two backbone restatements against each other (spconv is absent:
+"""CPU tier: pins the oracle restatement against golden vectors frozen from the reference's own files
+(tests/golden/ref_tiny.npz, ref_live.npz: oracle/make_golden*.py); checks the two backbone restatements against each other (spconv is absent:
 parity unpinned there) and the state-dict / C-ABI contracts."""
 import ctypes
 import os
@@ -11,10 +10,10 @@ import pytest
 import torch
 
 from oracle import pillarnext_oracle as O
-from oracle import reference_loader as RL
 from oracle.make_golden import golden_setup
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "ref_tiny.npz")
+GOLD_LIVE = os.path.join(os.path.dirname(__file__), "golden", "ref_live.npz")
 
 
 @pytest.fixture(scope="module")
@@ -59,7 +58,7 @@ def test_neck_head_loss_oracle_vs_golden(setup):
             assert abs(float(r[k]) - float(g["loss_t%d_%s" % (t, k)])) < 1e-4 * max(1.0, abs(float(g["loss_t%d_%s" % (t, k)]))), (t, k)
         assert np.abs(r["loc_loss_elem"].numpy() - g["loss_t%d_loc_elem" % t]).max() < 1e-5
     loss.backward()
-    for name, got in (("grad_head_x", xh.grad), ("grad_shared_conv_w", p["head.shared_conv.0.weight"].grad), ("grad_t1_hm_3_w", p["head.tasks.1.hm.3.weight"].grad)):
+    for name, got in (("grad_head_x", xh.grad), ("grad_shared_conv_w", p["head.shared_conv.0.weight"].grad[:16]), ("grad_t1_hm_3_w", p["head.tasks.1.hm.3.weight"].grad)):
         ref = g[name]
         assert np.abs(got.numpy() - ref).max() < 1e-4 * max(1e-3, np.abs(ref).max()), name
 
@@ -158,30 +157,26 @@ def test_product_never_imports_oracle():
                     assert not re.search(r"^\s*(from|import)\s+oracle\b", src, re.M), os.path.join(dp, f)
 
 
-@pytest.mark.skipif(not RL.available(), reason="reference tree not present")
 def test_oracle_and_synth_vs_live_reference(setup):
+    """The reference's AssignLabel, collate and PillarFeatureNet outputs on these inputs are stored in ref_live.npz."""
+    from oracle.make_golden_live import ASSIGN_KEYS
     from pillarnext_b200 import synth
     cfg, sd, ex, _, _, _ = setup
-    ref = RL.load_reference()
+    gold = np.load(GOLD_LIVE)
     # label assignment restatement (synth.assign_labels) vs reference AssignLabel + collate
     boxes, names = synth.make_gt(3, 25, cfg)
     mine = synth.assign_labels(boxes, names, cfg)
-    al = ref.AssignLabel(cfg["tasks"], 0.1, 500, 2, cfg["pc_range"], cfg["voxel_size"], cfg["out_size_factor"])
-    res = al({"annotations": {"gt_boxes": boxes, "gt_names": np.array(names)}})
-    for k in ("hm", "anno_box", "ind", "mask", "cat", "gt_boxes"):
+    for k in ASSIGN_KEYS:
         for t in range(len(cfg["tasks"])):
-            assert np.array_equal(np.nan_to_num(res[k][t], nan=-7.0), np.nan_to_num(mine[k][t], nan=-7.0)), (k, t)
+            want = gold["assign_%s_%d" % (k, t)]
+            assert np.array_equal(np.nan_to_num(want, nan=-7.0), np.nan_to_num(np.asarray(mine[k][t]), nan=-7.0)), (k, t)
     frames = [synth.make_frame(s, 300, cfg) for s in range(2)]
-    col = ref.collate([{"points": f} for f in frames])
-    assert torch.equal(col["points"], synth.collate_points(frames))
+    assert torch.equal(torch.from_numpy(gold["collate_points"]), synth.collate_points(frames))
     # a different seed / shape than the golden file: oracle reader vs the reference file
     pts = synth.collate_points([synth.make_frame(11, 2000, synth.NUSC, "lidar", sweeps=10)])
-    r = ref.PillarFeatureNet(5, [64, 64], synth.NUSC["voxel_size"], synth.NUSC["pc_range"])
-    r.load_state_dict({k[len("reader."):]: v.clone() for k, v in sd.items() if k.startswith("reader.")})
-    r.train()
-    f, c, _ = r(pts)
     f2, c2, _ = O.reader_forward(pts, sd, synth.NUSC["voxel_size"], synth.NUSC["pc_range"], train=True)
-    assert torch.equal(c, c2) and (f - f2).abs().max().item() < 2e-5
+    assert torch.equal(torch.from_numpy(gold["reader_coords"]), c2)
+    assert (torch.from_numpy(gold["reader_feat"]) - f2).abs().max().item() < 2e-5
 
 
 def test_convert_sync_batchnorm_is_honoured():

@@ -2,7 +2,7 @@
 
 BASELINE.json north_star: "boxes/heatmaps matching the reference within 1e-3 abs on identical inputs (voxel indices
 bit-exact)".  The reference is fp32 end to end; the production path stores bf16 activations and cannot meet 1e-3
-through 35 conv+BN layers.  In `precision("split")` every activation is a (hi, lo) bf16 pair and the SAME tcgen05
+through 35 conv+BN layers.  In `precision("split")` every activation is a (hi, lo) bf16 pair and the SAME wgmma
 kernels (pnx_igemm / pnx_wgrad over the (piece, piece) segments of 3-piece operands) run, so the assembled detector is
 compared here with the fp32 oracle at the stated tolerance: forward maps 1e-3 abs, parameter gradients 2e-3 rel-L2
 (fp32 summation-order level), and the bf16 path's measured error is printed next to it.

@@ -1,20 +1,22 @@
 """Oracle pinning for row F1 (decode + rotated NMS), CPU only.
 
-* oracle.predict_oracle.iou_bev  vs  the reference's own iou3d_cpu.cpp compiled into oracle/_ref (build container only;
-  on the GPU box the prebuilt oracle/_ref/*.so travels with the snapshot, otherwise the test is skipped);
+* oracle.predict_oracle.iou_bev  vs  the reference's own iou3d_cpu.cpp (its output on seeded boxes is stored in
+  tests/golden/ref_live.npz by oracle/make_golden_live.py);
 * oracle.predict_oracle.predict  vs  the reference's own CenterHead.predict run on CPU with its CUDA-only nms_gpu call
-  replaced by the oracle's greedy rotated NMS (needs /root/reference: build container only);
+  replaced by the oracle's greedy rotated NMS (outputs stored in tests/golden/ref_predict.npz);
 * closed-form IoU cases and NMS invariants that need neither.
 """
 import math
-import types
+import os
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import build_ref_iou, predict_oracle as P, reference_loader
+from oracle import predict_oracle as P
 from oracle.predict_fixtures import fake_preds as _fake_preds, test_cfg as _test_cfg, to_rows
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def rand_boxes(n, seed, spread=6.0):
@@ -40,12 +42,9 @@ def test_iou_closed_form():
 
 
 def test_iou_matches_reference_extension():
-    ext = build_ref_iou.load(build=True)
-    if ext is None:
-        pytest.skip("reference iou3d_cpu.cpp neither compiled (oracle/_ref) nor present")
+    """tests/golden/ref_live.npz holds the reference's boxes_iou_bev_cpu (iou3d_cpu.cpp) on these boxes."""
     a, b = rand_boxes(24, 1), rand_boxes(24, 2)
-    want = torch.zeros(24, 24)
-    ext.boxes_iou_bev_cpu(a.contiguous(), b.contiguous(), want)
+    want = torch.from_numpy(np.load(os.path.join(GOLDEN, "ref_live.npz"))["iou_bev"])
     got = torch.tensor([[float(P.iou_bev(x.numpy(), y.numpy())) for y in b] for x in a])
     assert (want > 0.05).sum() > 20                                        # the sample does overlap
     assert (got - want).abs().max().item() < 2e-5, (got - want).abs().max().item()
@@ -64,22 +63,13 @@ def test_nms_invariants():
 
 
 def test_predict_matches_reference_predict():
-    if not reference_loader.available():
-        pytest.skip("reference tree not present (build container only)")
-    ref = reference_loader.load_reference()
+    """tests/golden/ref_predict.npz holds the reference's CenterHead.predict on these inputs (oracle/make_golden_predict.py)."""
+    gold = np.load(os.path.join(GOLDEN, "ref_predict.npz"))
     tasks = [["car"], ["truck", "construction_vehicle"]]
-    head = ref.CenterHead(in_channels=256, tasks=tasks, weight=0.25, code_weights=[1.0] * 10,
-                          common_heads=dict(reg=[2, 2], height=[1, 2], dim=[3, 2], rot=[2, 2], vel=[2, 2]),
-                          strides=[2, 2], rectifier=[[0.0], [0.0, 0.0]])
     cfg = _test_cfg()
     preds = [_fake_preds(2, 24, 20, len(t), 10 + i) for i, t in enumerate(tasks)]
-    ns = lambda d: types.SimpleNamespace(**{k: (ns(v) if isinstance(v, dict) else v) for k, v in d.items()})
-    saved = ref.box_torch_ops.rotate_nms_pcdet
-    ref.box_torch_ops.rotate_nms_pcdet = P.rotate_nms_pcdet                # nms_gpu is CUDA-only: the oracle NMS stands in
-    try:
-        want = head.predict(dict(token=["a", "b"]), [{k: v.clone() for k, v in p.items()} for p in preds], ns(cfg))
-    finally:
-        ref.box_torch_ops.rotate_nms_pcdet = saved
+    want = [dict(token=tok, **{k: torch.from_numpy(gold["%s_%d" % (k, i)]) for k in ("box3d_lidar", "scores", "label_preds")})
+            for i, tok in enumerate(["a", "b"])]
     got = P.predict(preds, [len(t) for t in tasks], cfg, [[0.0], [0.0, 0.0]], tokens=["a", "b"])
     assert len(got) == len(want) == 2
     for g, w in zip(got, want):
@@ -130,9 +120,8 @@ def test_host_compiled_decode_and_iou_match_oracle():
 
 def test_oracle_predict_matches_golden_reference_outputs():
     """Runs anywhere: tests/golden/ref_predict.npz holds the reference's own predict outputs (oracle/make_golden_predict.py)."""
-    import os
     from oracle.make_golden_predict import SEEDS, SHAPE, TASKS
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_predict.npz")
+    path = os.path.join(GOLDEN, "ref_predict.npz")
     gold = np.load(path)
     preds = [_fake_preds(*SHAPE, len(t), SEEDS[i]) for i, t in enumerate(TASKS)]
     got = P.predict(preds, [len(t) for t in TASKS], _test_cfg(), [[0.0], [0.0, 0.0]], tokens=["a", "b"])
@@ -187,18 +176,14 @@ def test_host_compiled_decode_with_rectifier_and_iou_head():
 
 def test_iou_head_loss_oracle_matches_reference_loss():
     """Waymo-style head (extra `iou` head, with_reg_iou): the reference's own CenterHead.loss on CPU, with only the
-    CUDA-only boxes_aligned_iou3d_gpu swapped for the oracle's aligned IoU, against the oracle's center_loss(with_iou)."""
-    if not reference_loader.available():
-        pytest.skip("reference tree not present (build container only)")
+    CUDA-only boxes_aligned_iou3d_gpu swapped for the oracle's aligned IoU (stored in tests/golden/ref_live.npz by
+    oracle/make_golden_live.py, which builds the same inputs), against the oracle's center_loss(with_iou)."""
     from oracle import pillarnext_oracle as O
     from pillarnext_b200 import synth
-    ref = reference_loader.load_reference()
+    gold = np.load(os.path.join(GOLDEN, "ref_live.npz"))
     tasks = [["vehicle"], ["pedestrian", "cyclist"]]
     cfg = synth.tiny_config(64, tasks)
     heads = dict(reg=[2, 2], height=[1, 2], dim=[3, 2], rot=[2, 2], vel=[2, 2], iou=[1, 2])
-    head = ref.CenterHead(in_channels=256, tasks=tasks, weight=1.0, code_weights=cfg["code_weights"], common_heads=heads,
-                          strides=[2, 2], with_reg_iou=True, voxel_size=cfg["voxel_size"], pc_range=cfg["pc_range"],
-                          out_size_factor=[4, 4], rectifier=[[0.68], [0.71, 0.65]])
     ex = synth.make_batch([3, 4], 1500, cfg, n_boxes=12, sweeps=1)
     H = W = 64 // 8 * 2
     g = torch.Generator().manual_seed(5)
@@ -207,18 +192,11 @@ def test_iou_head_loss_oracle_matches_reference_loss():
         pd = {k: torch.randn(2, c, H, W, generator=g) * 0.5 for k, (c, _) in heads.items()}
         pd["hm"] = torch.randn(2, len(names), H, W, generator=g) - 2.0
         preds.append(pd)
-    fake = lambda a, b: torch.tensor([[float(P.aligned_iou3d(x.numpy(), y.numpy()))] for x, y in zip(a, b)],
-                                     dtype=a.dtype).reshape(-1, 1)
-    saved = ref.centerloss.boxes_aligned_iou3d_gpu
-    ref.centerloss.boxes_aligned_iou3d_gpu = fake
-    try:
-        want, want_logs = head.loss(ex, [{k: v.clone() for k, v in pd.items()} for pd in preds])
-    finally:
-        ref.centerloss.boxes_aligned_iou3d_gpu = saved
+    want = float(gold["iou_head_loss"][0])
     got, logs = O.center_loss(ex, preds, 1.0, cfg["code_weights"], True, cfg["voxel_size"], cfg["pc_range"], [4, 4],
                               with_iou=True)
-    assert abs(float(got) - float(want)) < 1e-5 * max(1.0, abs(float(want)))
+    assert abs(float(got) - want) < 1e-5 * max(1.0, abs(want))
     for t in range(2):
         assert float(ex["mask"][t].sum()) > 0
-        assert abs(float(logs[t]["iou_loss"]) - float(want_logs[t]["iou_loss"])) < 1e-6
+        assert abs(float(logs[t]["iou_loss"]) - float(gold["iou_head_iou_loss"][t])) < 1e-6
         assert 0.0 < float(logs[t]["iou_loss"]) < 2.0

@@ -1,4 +1,4 @@
-"""tcgen05 weight-gradient GEMM (MN-major operands) and the row-wise BatchNorm kernels vs torch fp32
+"""wgmma weight-gradient GEMM (MN-major operands) and the row-wise BatchNorm kernels vs torch fp32
 autograd on the same bf16-rounded operands.  Tolerance: 3e-3 of the result scale (fp32 accumulation
 order + fp32 atomics); BN backward additionally carries bf16 rounding of dx (2^-8 relative)."""
 import pytest
