@@ -7,11 +7,15 @@
 // Both operands are MN-major for the MMA (the reduction index K = row m is the slow one in memory):
 // tiles are staged as [64 rows x 128 B] blocks per 64-channel group with the 128-byte swizzle and
 // described to wgmma as transposed operands (LBO = block stride, SBO = 8-row group stride).
-// One CTA owns a 128-channel block of X, an NYC-channel chunk of Y and a GROUP of up to TG taps: the X tile of a
-// 64-row chunk is staged ONCE and multiplied against the gathered Y tile of every tap of the group, so the direct
-// operand is not re-read per tap (NYC * TG <= 256 register accumulator columns).
+// One CTA owns a 128-channel block of X, an NYC-channel chunk of Y and a GROUP of TG taps: the X tile of a 64-row chunk
+// is staged ONCE, and the group's Y tiles sit side by side as TG * NYC / 64 consecutive 64-channel atoms, so one
+// m64nNk16 wgmma with N = TG * NYC (<= 256 register accumulator columns) multiplies X against every tap of the group.
+// A group past the last tap is padded with zero tiles (every CTA of a launch runs the same N, with no branch around
+// the MMAs).  Accumulator column c is tap c / NYC, Y channel c % NYC.
 // Grid = (x blocks * y chunks, tap groups, K splits), two full waves of one CTA per SM.  Warpgroup 0: X by TMA, Y rows by
-// cp.async through a (tap, row) table; warpgroups 1-2: wgmma, then red.global.add (or a split's slab) from registers.
+// cp.async, each warp gathering the rows whose indices its lanes hold; warpgroups 1-2: wgmma, then a split's slab (or
+// red.global.add) from registers.  With a 64-channel X both consumer warpgroups multiply the one X block, each over
+// half of the group's columns.  Either way every dW element is one accumulator summing the split's rows in order.
 // This is the backward of: spconv SparseConv2d/SubMConv2d (reference sparse_conv.py:25-29,50-51),
 // nn.Conv2d/F.conv2d (aspp.py:19-32, conv.py:9-10, centerhead.py:35-46,108-114), nn.ConvTranspose2d
 // (centerhead.py:26-27) -- autograd derives these in the reference (trainer.py:94-108 loss.backward()).
@@ -31,7 +35,6 @@ struct WgradParams {
   float* dW;       // [T, X_total, Y_total]
   float* partials; // deterministic mode: [splits][T, X_total, Y_total], plain stores, reduced in split order afterwards
   int X_total, Y_total;
-  int x_dup;       // X has only 64 channels: the second consumer warpgroup has no X channels
   int y_chunks;    // Y_total / NYC
   int taps_per_group;
   int rows_per_split;
@@ -41,33 +44,36 @@ constexpr int kThreads = 384;         // producer warpgroup + two consumer warpg
 constexpr int kKS = 64;               // rows (K) per stage
 constexpr uint32_t kBlk = kKS * 128;  // bytes of one [64 rows x 64 ch] block
 
-// NYC = Y channels per CTA (64..256), TG = max taps per group (NYC * TG <= 256 accumulator columns)
-template <int NYC, int TG>
+// NYC = Y channels per CTA (64..256), TG = taps per group: one MMA per k16 step spans the N = NYC * TG columns of the
+// group.  XD (X has 64 channels): both consumer warpgroups multiply the one X block, each over half of the columns.
+template <int NYC, int TG, bool XD>
 struct WCfg {
+  static constexpr int kN = NYC * TG;
+  static constexpr int kNW = XD ? kN / 2 : kN;  // accumulator columns of one consumer warpgroup
   static constexpr int kYAtoms = NYC / 64;
   static constexpr uint32_t kStageBytes = (2 + TG * kYAtoms) * kBlk;
   static constexpr int kStagesRaw = (200 * 1024) / (int)kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr size_t kSmem = 1024 + (size_t)kStages * kStageBytes + 256 + (size_t)TG * kKS * 4;
-  static_assert(NYC * TG <= 256, "register accumulator budget");
+  static constexpr size_t kSmem = 1024 + (size_t)kStages * kStageBytes + 256;
+  static_assert(kN <= 256 && (kNW == 64 || kNW == 128 || kNW == 192 || kNW == 256), "one wgmma shape, <= 256 register accumulator columns");
+  static_assert(!XD || kN % 128 == 0, "a warpgroup's half of the columns is whole 64-channel atoms");
   static_assert(kStages >= 2, "need at least two stages");
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
 
-template <int NYC, int TG>
+template <int NYC, int TG, bool XD>
 __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constant__ CUtensorMap xmap, WgradParams p) {
-  using C = WCfg<NYC, TG>;
-  constexpr int kStages = C::kStages, kYAtoms = C::kYAtoms;
+  using C = WCfg<NYC, TG, XD>;
+  constexpr int kStages = C::kStages, kYAtoms = C::kYAtoms, kNW = C::kNW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)kStages * C::kStageBytes);
   uint64_t* empty = full + kStages;
-  int* s_idx = reinterpret_cast<int*>(smem + (size_t)kStages * C::kStageBytes + 256);  // [TG][kKS] gathered row (-1 = absent)
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int xb = blockIdx.x / p.y_chunks, yc = blockIdx.x - xb * p.y_chunks;
   const int t0 = blockIdx.y * p.taps_per_group;
-  const int ntaps = min(p.taps_per_group, p.T - t0);
+  const int ntaps = min(TG, p.T - t0);  // taps [ntaps, TG) of the group are zero tiles
   const int split = blockIdx.z;
   const int m_begin = split * p.rows_per_split;
   const int m_end = min(p.M, m_begin + p.rows_per_split);
@@ -81,26 +87,34 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constan
     }
     pnx::fence_barrier_init();
   }
+  if (ntaps < TG) {
+    // the Y tiles of the padding taps are zeroed once in every stage and never written again
+    constexpr int kPer = kBlk / 16;  // 16-byte words of one block
+    const int pad_words = (TG - ntaps) * kYAtoms * kPer;
+    for (int i = threadIdx.x; i < kStages * pad_words; i += kThreads) {
+      const int s = i / pad_words, w = i - s * pad_words;
+      *reinterpret_cast<uint4*>(smem + (size_t)s * C::kStageBytes + (2 + ntaps * kYAtoms) * kBlk + (size_t)w * 16) = make_uint4(0, 0, 0, 0);
+    }
+    pnx::fence_proxy_async_smem();  // written through the generic proxy, read by wgmma
+  }
   __syncthreads();
   if (num_k <= 0) return;
 
   if (wg == 0) {
     // ---------------------------------------------------------------- producer
     pnx::regs_dealloc<56>();
-    const int ptid = threadIdx.x;
+    const int warp = threadIdx.x >> 5;
     const int y_ch0 = yc * NYC;
-    const int nchunks = ntaps * kYAtoms * kKS * 8;  // 16-byte copies of Y per stage
-    const int nblk = p.x_dup ? 1 : 2;
+    const int nblk = XD ? 1 : 2;
     const int hw = p.Hout * p.Wout;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int kc = 0; kc < num_k; ++kc) {
-      const int mb = m_begin + kc * kKS;
-      // gathered row of (tap j, row r) for e = j * 64 + r
-      int val[(TG * kKS + 127) / 128];
+    // Warp w gathers rows [16 w, +16) of every tap of the group.  Lane l holds the Y row of (tap 2 n + l / 16,
+    // row 16 w + l % 16) in idx[n] (-1 = absent: zero fill) and hands it to the lanes copying that row with a shuffle.
+    constexpr int kIdxRegs = (TG + 1) / 2;
+    auto load_idx = [&](int kc, int (&idx)[kIdxRegs]) {
+      const int m = m_begin + kc * kKS + 16 * warp + (lane & 15);
 #pragma unroll
-      for (int n = 0; n < (TG * kKS + 127) / 128; ++n) {
-        const int e = n * 128 + ptid, j = e >> 6, m = mb + (e & (kKS - 1));
+      for (int n = 0; n < kIdxRegs; ++n) {
+        const int j = 2 * n + (lane >> 4);
         int g = -1;
         if (j < ntaps && m < m_end) {
           const int t = t0 + j;
@@ -119,88 +133,89 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constan
             }
           }
         }
-        val[n] = g;
+        idx[n] = g;
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // the previous chunk's table has been read
-#pragma unroll
-      for (int n = 0; n < (TG * kKS + 127) / 128; ++n)
-        if (n * 128 + ptid < TG * kKS) s_idx[n * 128 + ptid] = val[n];
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+    };
+    int idx[kIdxRegs], nxt[kIdxRegs];
+    load_idx(0, idx);
+    // a warp instruction copies 4 whole 128-byte rows 16 w + 4 qq + rq; their swizzle depends only on rq and qq & 1
+    const int sub = lane & 7, rq = lane >> 3;
+    const uint32_t row_off = (uint32_t)(16 * warp + rq) * 128;
+    const uint32_t swz[2] = {(uint32_t)(sub ^ rq) << 4, (uint32_t)(sub ^ (rq + 4)) << 4};
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kc = 0; kc < num_k; ++kc) {
+      if (kc + 1 < num_k) load_idx(kc + 1, nxt);  // the next stage's indices load while this one waits for its slot
       pnx::mbar_wait(&empty[stage], phase ^ 1);
       uint8_t* st = smem + (size_t)stage * C::kStageBytes;
-      if (ptid == 0) {
+      if (threadIdx.x == 0) {
         // X: plain 2-D TMA boxes of [64 rows x 64 channels] (rows past M are zero-filled by the tensor map bounds)
         pnx::mbar_arrive_expect_tx(&full[stage], (uint32_t)nblk * kBlk);
-        for (int b2 = 0; b2 < nblk; ++b2) pnx::tma_load_2d(&xmap, &full[stage], st + b2 * kBlk, xb * 128 + b2 * 64, mb);
+        for (int b2 = 0; b2 < nblk; ++b2) pnx::tma_load_2d(&xmap, &full[stage], st + b2 * kBlk, xb * 128 + b2 * 64, m_begin + kc * kKS);
       }
-      const uint32_t sy = pnx::smem_u32(st) + 2 * kBlk;
-      for (int c = ptid; c < nchunks; c += 128) {  // a warp instruction copies 4 whole 128-byte rows
-        const int sub = c & 7, row = (c >> 3) & (kKS - 1), blk = c >> 9;  // blk = tap * kYAtoms + atom
-        const int tap = blk / kYAtoms, atom = blk - tap * kYAtoms;
-        const int g = s_idx[tap * kKS + row];
-        const __nv_bfloat16* src = p.Y + (long long)(g < 0 ? 0 : g) * p.ldy + y_ch0 + atom * 64 + sub * 8;
-        pnx::cp_async_16(sy + blk * kBlk + pnx::sw128_offset(row, sub), src, g < 0 ? 0u : 16u);
+      const uint32_t sy = pnx::smem_u32(st) + 2 * kBlk + row_off;
+#pragma unroll
+      for (int j = 0; j < TG; ++j) {
+        if (j >= ntaps) break;  // padding taps stay zero
+#pragma unroll
+        for (int qq = 0; qq < 4; ++qq) {
+          const int g = __shfl_sync(0xffffffffu, idx[j >> 1], ((j & 1) << 4) + 4 * qq + rq);
+          const __nv_bfloat16* src = p.Y + (long long)(g < 0 ? 0 : g) * p.ldy + y_ch0 + sub * 8;
+#pragma unroll
+          for (int a = 0; a < kYAtoms; ++a)
+            pnx::cp_async_16(sy + (j * kYAtoms + a) * kBlk + qq * 512 + swz[qq & 1], src + a * 64, g < 0 ? 0u : 16u);
+        }
       }
       pnx::cp_async_mbar_arrive(&full[stage]);
+#pragma unroll
+      for (int n = 0; n < kIdxRegs; ++n) idx[n] = nxt[n];
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
   } else {
-    // ---------------------------------------------------------------- consumers: X channels [64 * half, +64) of the block
+    // ---------------------------------------------------------------- consumers
+    // X channels [64 * half, +64) of the block over all columns, or (XD) the one X block over columns [kNW * half, +kNW)
     pnx::regs_alloc<224>();
     const int half = wg - 1;
-    const bool mine = !(p.x_dup && half == 1);
-    float acc[TG][NYC / 2];
+    const uint32_t x_off = XD ? 0u : (uint32_t)half * kBlk;
+    const uint32_t y_off = 2 * kBlk + (XD ? (uint32_t)half * (kNW / 64) * kBlk : 0u);
+    float acc[kNW / 2];
 #pragma unroll
-    for (int j = 0; j < TG; ++j)
-#pragma unroll
-      for (int i = 0; i < NYC / 2; ++i) acc[j][i] = 0.f;
+    for (int i = 0; i < kNW / 2; ++i) acc[i] = 0.f;
     int stage = 0, prev = 0;
     uint32_t phase = 0;
     for (int kc = 0; kc < num_k; ++kc) {
       pnx::mbar_wait(&full[stage], phase);
       pnx::fence_proxy_async_smem();  // the cp.async rows were written through the generic proxy; wgmma reads async
-      if (mine) {
-        pnx::wgmma_fence();
+      pnx::wgmma_fence();
+      pnx::fence_acc(acc);
+      const uint32_t st = pnx::smem_u32(smem + (size_t)stage * C::kStageBytes);
 #pragma unroll
-        for (int j = 0; j < TG; ++j) pnx::fence_acc(acc[j]);
-        const uint32_t sx = pnx::smem_u32(smem + (size_t)stage * C::kStageBytes) + half * kBlk;
-        const uint32_t sy = pnx::smem_u32(smem + (size_t)stage * C::kStageBytes) + 2 * kBlk;
-#pragma unroll
-        for (int k = 0; k < kKS / 16; ++k) {
-          const uint64_t dx = pnx::make_smem_desc_sw128(sx + k * 2048, kBlk, 1024);
-#pragma unroll
-          for (int j = 0; j < TG; ++j)
-            if (j < ntaps)
-              pnx::Wgmma<NYC, 1, 1>::mma(acc[j], dx, pnx::make_smem_desc_sw128(sy + j * kYAtoms * kBlk + k * 2048, kBlk, 1024),
-                                         (kc > 0 || k > 0) ? 1u : 0u);
-        }
-        pnx::wgmma_commit();
-        pnx::wgmma_wait<1>();
-      }
+      for (int k = 0; k < kKS / 16; ++k)
+        pnx::Wgmma<kNW, 1, 1>::mma(acc, pnx::make_smem_desc_sw128(st + x_off + k * 2048, kBlk, 1024),
+                                   pnx::make_smem_desc_sw128(st + y_off + k * 2048, kBlk, 1024), (kc > 0 || k > 0) ? 1u : 0u);
+      pnx::wgmma_commit();
+      pnx::wgmma_wait<1>();  // the previous stage's MMAs are done: release it
       if (kc > 0 && lane == 0) pnx::mbar_arrive(&empty[prev]);
       prev = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-    if (!mine) return;
     pnx::wgmma_wait<0>();
-#pragma unroll
-    for (int j = 0; j < TG; ++j) pnx::fence_acc(acc[j]);
-    // ---------------------------------------------------------------- epilogue: registers -> red.global.add
+    pnx::fence_acc(acc);
+    // ---------------------------------------------------------------- epilogue: registers -> the split's slab
     float* out = p.partials ? p.partials + (size_t)blockIdx.z * ((size_t)p.T * p.X_total * p.Y_total) : p.dW;
+    const int x0 = xb * 128 + (XD ? 0 : half * 64);
+    const int c0 = XD ? half * kNW : 0;
 #pragma unroll
-    for (int j = 0; j < TG; ++j) {
-      if (j >= ntaps) break;
-#pragma unroll
-      for (int i = 0; i < NYC / 2; i += 2) {
-        const int xch = xb * 128 + half * 64 + pnx::acc_row(i);
-        if (xch >= p.X_total) continue;
-        float* dst = out + ((size_t)(t0 + j) * p.X_total + xch) * p.Y_total + yc * NYC + pnx::acc_col(i);
-        if (p.partials) {  // every (tap, x, y) of a split's slab is written by exactly one CTA
-          *reinterpret_cast<float2*>(dst) = make_float2(acc[j][i], acc[j][i + 1]);
-        } else {
-          atomicAdd(dst, acc[j][i]);
-          atomicAdd(dst + 1, acc[j][i + 1]);
-        }
+    for (int i = 0; i < kNW / 2; i += 2) {
+      const int c = c0 + pnx::acc_col(i), j = c / NYC;
+      const int xch = x0 + pnx::acc_row(i);
+      if (j >= ntaps || xch >= p.X_total) continue;  // padding taps are not stored
+      float* dst = out + ((size_t)(t0 + j) * p.X_total + xch) * p.Y_total + yc * NYC + (c - j * NYC);
+      if (p.partials) {  // every (tap, x, y) of a split's slab is written by exactly one CTA
+        *reinterpret_cast<float2*>(dst) = make_float2(acc[i], acc[i + 1]);
+      } else {
+        atomicAdd(dst, acc[i]);
+        atomicAdd(dst + 1, acc[i + 1]);
       }
     }
   }
@@ -215,52 +230,60 @@ __global__ void wgrad_reduce_partials_kernel(const float* __restrict__ partials,
   }
 }
 
-// grid plan shared by the launcher and pnx_wgrad_splits
-struct WPlan { int taps_per_group, groups, rows_per_split, splits; };
-inline WPlan wgrad_plan(int TG, int NYC, int x_blocks, int Y_total, int T, int M, int sm_count) {
-  WPlan w;
-  const int y_chunks = Y_total / NYC;
-  w.taps_per_group = T < TG ? T : TG;
-  w.groups = (T + w.taps_per_group - 1) / w.taps_per_group;
-  w.taps_per_group = (T + w.groups - 1) / w.groups;  // balance the groups (e.g. 9 taps, TG = 8 -> 5 + 4)
-  w.groups = (T + w.taps_per_group - 1) / w.taps_per_group;
-  const int ctas_xy = x_blocks * y_chunks * w.groups;
+// the (NYC, TG) variant pnx_wgrad picks for a shape: the largest Y chunk of 256/192/128/64 dividing y_channels; the taps
+// of a 128- or 64-channel chunk are grouped so that one MMA spans N = 192 or 256 columns (3 x 3: 5 groups of 2 taps at
+// 128 channels, 3 groups of 3 at 64; ConvTranspose 2 x 2 at 64: one group of 4), with the fewest zero padding taps.
+// XD (64-channel X): each consumer warpgroup takes half of the N columns, so N is 128 or 256 (whole atoms per half);
+// 3 x 3 at 64 Y channels then runs 3 groups of 4 taps, the last one 1 tap + 3 padding taps.
+inline void wgrad_variant(int y_channels, int taps, bool xd, int* NYC, int* TG) {
+  if (xd) {
+    if (y_channels % 256 == 0) { *NYC = 256; *TG = 1; }
+    else if (y_channels % 128 == 0) { *NYC = 128; *TG = taps > 1 ? 2 : 1; }
+    else { *NYC = 64; *TG = taps <= 2 ? 2 : 4; }
+    return;
+  }
+  if (y_channels % 256 == 0) { *NYC = 256; *TG = 1; }
+  else if (y_channels % 192 == 0) { *NYC = 192; *TG = 1; }
+  else if (y_channels % 128 == 0) { *NYC = 128; *TG = taps > 1 ? 2 : 1; }
+  else { *NYC = 64; *TG = taps == 1 ? 1 : (4 - taps % 4) % 4 <= (3 - taps % 3) % 3 ? 4 : 3; }
+}
+
+// K split plan shared by the launcher and pnx_wgrad_splits.  It depends on the shape alone (it is sized from the grid of
+// the full-X-block variant, whatever variant runs), so the order in which every dW element is summed -- the rows of a
+// split in order, then the splits in order -- does not depend on how the taps and Y channels are tiled.
+struct WPlan { int rows_per_split, splits; };
+inline WPlan wgrad_plan(int x_blocks, int Y_total, int T, int M, int sm_count) {
+  int NYC, TG;
+  wgrad_variant(Y_total, T, false, &NYC, &TG);
+  const int ctas_xy = x_blocks * (Y_total / NYC) * ((T + TG - 1) / TG);
   // two full waves of CTAs (one CTA per SM): round DOWN -- 2*132 + a few CTAs would run a third, nearly empty wave
   int splits = (2 * sm_count) / ctas_xy;
   const int max_splits = (M + 8 * kKS - 1) / (8 * kKS);  // at least 8 K-chunks per CTA
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
+  WPlan w;
   w.rows_per_split = ((M + splits - 1) / splits + kKS - 1) / kKS * kKS;
   w.splits = (M + w.rows_per_split - 1) / w.rows_per_split;
   return w;
 }
-// the (NYC, TG) variant pnx_wgrad picks for a shape: the largest Y chunk of 256/192/128/64 dividing y_channels, taps per
-// group bounded by the 256 accumulator columns
-inline void wgrad_variant(int y_channels, int* NYC, int* TG) {
-  if (y_channels % 256 == 0) { *NYC = 256; *TG = 1; }
-  else if (y_channels % 192 == 0) { *NYC = 192; *TG = 1; }
-  else if (y_channels % 128 == 0) { *NYC = 128; *TG = 2; }
-  else { *NYC = 64; *TG = 4; }
-}
 
-template <int NYC, int TG>
+template <int NYC, int TG, bool XD>
 int launch_wgrad(const CUtensorMap& xmap, WgradParams p, int x_blocks, int sm_count, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    PNX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NYC, TG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WCfg<NYC, TG>::kSmem));
+    PNX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NYC, TG, XD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WCfg<NYC, TG, XD>::kSmem));
     attr_set = true;
   }
-  const WPlan w = wgrad_plan(TG, NYC, x_blocks, p.Y_total, p.T, p.M, sm_count);
+  const WPlan w = wgrad_plan(x_blocks, p.Y_total, p.T, p.M, sm_count);
   p.y_chunks = p.Y_total / NYC;
-  p.taps_per_group = w.taps_per_group;
+  p.taps_per_group = TG;
   p.rows_per_split = w.rows_per_split;
-  const int groups = w.groups, splits = w.splits;
-  dim3 grid(x_blocks * p.y_chunks, groups, splits);
-  wgrad_kernel<NYC, TG><<<grid, kThreads, WCfg<NYC, TG>::kSmem, stream>>>(xmap, p);
+  dim3 grid(x_blocks * p.y_chunks, (p.T + TG - 1) / TG, w.splits);
+  wgrad_kernel<NYC, TG, XD><<<grid, kThreads, WCfg<NYC, TG, XD>::kSmem, stream>>>(xmap, p);
   PNX_CHECK_LAUNCH();
   if (p.partials) {
     const long long n = (long long)p.T * p.X_total * p.Y_total;
-    wgrad_reduce_partials_kernel<<<(int)((n + 255) / 256 < 592 ? (n + 255) / 256 : 592), 256, 0, stream>>>(p.partials, splits, n, p.dW);
+    wgrad_reduce_partials_kernel<<<(int)((n + 255) / 256 < 592 ? (n + 255) / 256 : 592), 256, 0, stream>>>(p.partials, w.splits, n, p.dW);
     PNX_CHECK_LAUNCH();
   }
   return PNX_OK;
@@ -272,9 +295,7 @@ int launch_wgrad(const CUtensorMap& xmap, WgradParams p, int x_blocks, int sm_co
 extern "C" int pnx_wgrad_splits(int x_channels, int y_channels, int taps, int M, int sm_count) {
   if (M <= 0 || x_channels <= 0 || y_channels <= 0 || taps <= 0) return 0;
   if (sm_count <= 0) sm_count = 132;
-  int NYC, TG;
-  wgrad_variant(y_channels, &NYC, &TG);
-  return wgrad_plan(TG, NYC, x_channels == 64 ? 1 : x_channels / 128, y_channels, taps, M, sm_count).splits;
+  return wgrad_plan(x_channels == 64 ? 1 : x_channels / 128, y_channels, taps, M, sm_count).splits;
 }
 
 // Contract: include/pnx.h (pnx_wgrad).  dW must be zeroed (or hold the value to accumulate into).
@@ -298,7 +319,6 @@ extern "C" int pnx_wgrad(const void* X, long long ldx, int x_channels, const voi
   p.kw = kw > 0 ? kw : 1; p.mul = mul; p.dil = dil; p.pad = pad; p.shuffle = shuffle;
   p.dW = dW; p.partials = partials; p.X_total = x_channels; p.Y_total = y_channels;
   PNX_CHECK_ARG(!partials || (reinterpret_cast<uintptr_t>(partials) & 15) == 0, "partials 16-byte aligned");
-  p.x_dup = x_channels == 64 ? 1 : 0;
   p.y_chunks = 1; p.taps_per_group = 1; p.rows_per_split = M;
   const int x_blocks = x_channels == 64 ? 1 : x_channels / 128;
   PNX_CHECK_ARG((reinterpret_cast<uintptr_t>(X) & 15) == 0 && (reinterpret_cast<uintptr_t>(Y) & 15) == 0, "X/Y 16-byte aligned");
@@ -307,9 +327,17 @@ extern "C" int pnx_wgrad(const void* X, long long ldx, int x_channels, const voi
   if (rc) return rc;
   PNX_CHECK_ARG(y_rows >= 1 && y_rows < 0x7fffffffLL, "y_rows = number of rows of Y");
   int NYC, TG;
-  wgrad_variant(y_channels, &NYC, &TG);
-  if (NYC == 256) return launch_wgrad<256, 1>(xmap, p, x_blocks, sm_count, stream);
-  if (NYC == 192) return launch_wgrad<192, 1>(xmap, p, x_blocks, sm_count, stream);
-  if (NYC == 128) return launch_wgrad<128, 2>(xmap, p, x_blocks, sm_count, stream);
-  return launch_wgrad<64, 4>(xmap, p, x_blocks, sm_count, stream);
+  if (x_channels == 64) {
+    wgrad_variant(y_channels, taps, true, &NYC, &TG);
+    if (NYC == 256) return launch_wgrad<256, 1, true>(xmap, p, x_blocks, sm_count, stream);
+    if (NYC == 128) return TG == 2 ? launch_wgrad<128, 2, true>(xmap, p, x_blocks, sm_count, stream) : launch_wgrad<128, 1, true>(xmap, p, x_blocks, sm_count, stream);
+    return TG == 4 ? launch_wgrad<64, 4, true>(xmap, p, x_blocks, sm_count, stream) : launch_wgrad<64, 2, true>(xmap, p, x_blocks, sm_count, stream);
+  }
+  wgrad_variant(y_channels, taps, false, &NYC, &TG);
+  if (NYC == 256) return launch_wgrad<256, 1, false>(xmap, p, x_blocks, sm_count, stream);
+  if (NYC == 192) return launch_wgrad<192, 1, false>(xmap, p, x_blocks, sm_count, stream);
+  if (NYC == 128) return TG == 2 ? launch_wgrad<128, 2, false>(xmap, p, x_blocks, sm_count, stream) : launch_wgrad<128, 1, false>(xmap, p, x_blocks, sm_count, stream);
+  if (TG == 4) return launch_wgrad<64, 4, false>(xmap, p, x_blocks, sm_count, stream);
+  if (TG == 3) return launch_wgrad<64, 3, false>(xmap, p, x_blocks, sm_count, stream);
+  return launch_wgrad<64, 1, false>(xmap, p, x_blocks, sm_count, stream);
 }
