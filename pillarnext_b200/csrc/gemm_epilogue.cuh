@@ -124,7 +124,156 @@ __device__ __forceinline__ void gemm_epilogue(const float (&acc)[BN / 2], const 
   }
 }
 
-// after the last tile and a barrier of the consumer threads: per-warp sums, added in warp order, into the fp64 accumulators
+// ------------------------------------------------------------------ staged epilogue (F = 0, 1)
+// The consumer warpgroups only round the tile to bf16 into a shared staging buffer and go straight back to their MMAs;
+// store warps drain it while the next tile's mainloop runs: the BatchNorm statistics (or, F = 1, the BN-backward gate and
+// its sums) and coalesced 16-byte row stores.  A tile is staged in P passes of BN / P columns when one buffer for the
+// whole tile would leave too few pipeline stages.  F = 2 and igemm at BN = 256 keep the in-register epilogue above.
+template <int BN, int P>
+struct Staging {
+  static_assert(BN % P == 0 && (BN / P) % 8 == 0, "staging pass width");
+  static constexpr int kCols = BN / P;
+  static constexpr int kPitch = 2 * kCols + 16;  // bytes per staged row; the pad keeps the fragment stores conflict-free
+  static constexpr int kBytes = 128 * kPitch;
+};
+
+// consumer half: rows [64 * half, +64) of the tile, bf16(relu(acc + bias + addend)) into the staging buffer, pass by pass.
+// `staged` counts the 256 consumer threads; `sfree` is released by the store warps; spass counts passes over all tiles.
+template <int BN, int P>
+__device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BN / 2], const EpiParams& e, long long row_base, int nvalid,
+                                                    int half, int n0, const float* s_bias, uint8_t* stg, uint64_t* staged,
+                                                    uint64_t* sfree, uint32_t& spass) {
+  using S = Staging<BN, P>;
+  const int lane = threadIdx.x & 31;
+  const int lr0 = half * 64 + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+#pragma unroll
+  for (int pp = 0; pp < P; ++pp) {
+    mbar_wait(sfree, (spass & 1) ^ 1);
+#pragma unroll
+    for (int jj = 0; jj < S::kCols / 8; ++jj) {
+      const int j = pp * (S::kCols / 8) + jj;
+      const int c = 8 * j + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int lr = lr0 + 8 * h;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (e.has_bias) { v0 += s_bias[c]; v1 += s_bias[c + 1]; }
+        if (e.addend && lr < nvalid) {
+          const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(e.addend + (row_base + lr) * e.ld_add + n0 + c));
+          v0 += a.x; v1 += a.y;
+        }
+        if (e.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        *reinterpret_cast<__nv_bfloat162*>(stg + lr * S::kPitch + (c - pp * S::kCols) * 2) = __floats2bfloat162_rn(v0, v1);
+      }
+    }
+    mbar_arrive(staged);
+    ++spass;
+  }
+}
+
+// store half, run by `nthreads` threads (a multiple of 32, named barrier `bar_id`) for every tile the consumers stage.
+// The statistics of warp slot w (rows 16w .. 16w + 15) are summed exactly as the in-register epilogue sums them: the pair
+// of rows (g, g + 8), then ((t0 + t1) + (t2 + t3)) + ((t4 + t5) + (t6 + t7)) over the 8 row groups g, then into
+// s_stat[w] in tile order -- so the statistics are bit-identical to it.
+template <int BN, int F, int P>
+__device__ __forceinline__ void gemm_epilogue_drain(const EpiParams& e, long long row_base, int nvalid, int n0, uint8_t* stg,
+                                                    float* s_stat, const float* s_bnc, uint64_t* staged, uint64_t* sfree,
+                                                    uint32_t& spass, int tid, int nthreads, int bar_id) {
+  using S = Staging<BN, P>;
+  constexpr int kPairs = S::kCols / 2, kChunks = S::kCols / 8;
+  const bool want_stats = F == 1 || e.stats != nullptr;
+  if (F == 1) {  // raw does not depend on the MMAs: pull the tile's rows into L2 while the consumers still compute it
+    constexpr int kLines = BN / 64;  // 128-byte lines per row
+    for (int i = tid; i < nvalid * kLines; i += nthreads) {
+      const int r = i / kLines, l = i - r * kLines;
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(e.bnr_raw + (row_base + r) * e.bnr_ld + n0 + 64 * l));
+    }
+  }
+  for (int pp = 0; pp < P; ++pp) {
+    mbar_wait(staged, spass & 1);
+    if (want_stats) {
+      for (int it = tid; it < 8 * kPairs; it += nthreads) {
+        const int w = it / kPairs, pr = it - w * kPairs;
+        const int c = pp * S::kCols + 2 * pr;  // column pair (c, c + 1) inside the CTA's column block
+        const int gc = n0 + c;
+        // F = 1: the raw pairs of row groups [g0, g0 + 4), both halves, loaded together ahead of their use
+        uint32_t raw2[8];
+        auto load_raw = [&](int g0) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int lr = 16 * w + g0 + (i & 3) + 8 * (i >> 2);
+            raw2[i] = lr < nvalid ? __ldg(reinterpret_cast<const unsigned int*>(e.bnr_raw + (row_base + lr) * e.bnr_ld + gc)) : 0u;
+          }
+        };
+        // sums over the rows (16w + g, 16w + g + 8) of the column pair: s0, s1, q0, q1
+        auto rows = [&](int g) {
+          float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int lr = 16 * w + g + 8 * h;
+            if (lr < nvalid) {
+              __nv_bfloat162* sp = reinterpret_cast<__nv_bfloat162*>(stg + lr * S::kPitch + 4 * pr);
+              const float2 r = __bfloat1622float2(*sp);
+              if (F == 1) {
+                const float2 raw = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw2[(g & 3) + 4 * h]));
+                const float g0 = fmaf(raw.x, s_bnc[c], s_bnc[BN + c]) > 0.f ? r.x : 0.f;
+                const float g1 = fmaf(raw.y, s_bnc[c + 1], s_bnc[BN + c + 1]) > 0.f ? r.y : 0.f;
+                *sp = __floats2bfloat162_rn(g0, g1);
+                t.x += g0; t.y += g1;
+                t.z = fmaf(g0, (raw.x - s_bnc[2 * BN + c]) * s_bnc[3 * BN + c], t.z);
+                t.w = fmaf(g1, (raw.y - s_bnc[2 * BN + c + 1]) * s_bnc[3 * BN + c + 1], t.w);
+              } else {
+                t.x += r.x; t.y += r.y;
+                t.z = fmaf(r.x, r.x, t.z); t.w = fmaf(r.y, r.y, t.w);
+              }
+            }
+          }
+          return t;
+        };
+        auto add = [](float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); };
+        if (F == 1) load_raw(0);
+        float4 lo = add(rows(0), rows(1));
+        lo = add(lo, add(rows(2), rows(3)));
+        if (F == 1) load_raw(4);
+        float4 hi = add(rows(4), rows(5));
+        hi = add(hi, add(rows(6), rows(7)));
+        const float4 s = add(lo, hi);
+        if (F != 1 && e.stats_direct) {  // order-insensitive fp64 accumulation (see pnx_set_deterministic)
+          const int ch0 = gc % e.stats_mod, ch1 = (gc + 1) % e.stats_mod;
+          atomicAdd(&e.stats[ch0], (double)s.x); atomicAdd(&e.stats[ch1], (double)s.y);
+          atomicAdd(&e.stats[e.stats_C + ch0], (double)s.z); atomicAdd(&e.stats[e.stats_C + ch1], (double)s.w);
+        } else {
+          float* s_mine = s_stat + w * 2 * BN;
+          s_mine[c] += s.x; s_mine[c + 1] += s.y;
+          s_mine[BN + c] += s.z; s_mine[BN + c + 1] += s.w;
+        }
+      }
+      if (F == 1) asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(nthreads) : "memory");  // the gated values are staged
+    }
+    for (int idx = tid; idx < 128 * kChunks; idx += nthreads) {
+      const int r = idx / kChunks, ch = idx - r * kChunks;
+      if (r >= nvalid) break;
+      const uint4 v = *reinterpret_cast<const uint4*>(stg + r * S::kPitch + ch * 16);
+      const int gc = n0 + pp * S::kCols + ch * 8;
+      long long orow = row_base + r;
+      int ocol = gc;
+      if (e.shuffle) {
+        const int hw = e.Hout * e.Wout;
+        const int b = (int)(orow / hw), rem = (int)(orow - (long long)b * hw);
+        const int y = rem / e.Wout, x = rem - y * e.Wout;
+        const int q = gc >> 6;
+        orow = ((long long)(b * 2 * e.Hout + 2 * y)) * (2 * e.Wout) + 2 * x + (long long)(q >> 1) * (2 * e.Wout) + (q & 1);
+        ocol = gc & 63;
+      }
+      *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(e.out) + orow * e.ldc + ocol) = v;
+    }
+    mbar_arrive(sfree);
+    ++spass;
+  }
+}
+
+// after the last tile and a barrier of the threads that own s_stat: per-warp sums, added in warp order, into the fp64
+// accumulators
 template <int BN, int F>
 __device__ __forceinline__ void gemm_epilogue_flush(const EpiParams& e, int n0, const float* s_stat, double* bnr_red, int bnr_C,
                                                     int tid, int nthreads) {

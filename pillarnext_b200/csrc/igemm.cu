@@ -8,10 +8,13 @@
 //     centerhead.py:35-46,108-114): rows = pixels of a channels-last image, nbr computed from geometry
 //     (zero padding = absent neighbour), ConvTranspose2d k2 s2 (centerhead.py:26-27) = one GEMM with
 //     N = 4*Cout and a pixel-shuffle store.
-// CTA = 3 warpgroups, persistent over 128-row tiles: warpgroup 0 writes the gathered row of every (tap, row) of a tile
-// into shared memory, then per K stage loads the weight tile by TMA and gathers the 128 A rows with 16-byte cp.async
-// (index -1 = zero fill) into the 128B-swizzled layout; warpgroups 1-2 each run wgmma on 64 rows into registers and
-// apply the epilogue (gemm_epilogue.cuh).
+// CTA persistent over 128-row tiles: warpgroup 0 writes the gathered row of every (tap, row) of a tile into shared
+// memory, then per K stage loads the weight tile by TMA and gathers the 128 A rows with 16-byte cp.async (index -1 = zero
+// fill) into the 128B-swizzled layout; warpgroups 1-2 each run wgmma on 64 rows into registers.  Staged variants
+// (Cfg::kStaged) have a fourth warpgroup: the consumers round the tile into shared memory and go back to their MMAs, and
+// warpgroup 3 stores it and sums its statistics meanwhile (gemm_epilogue.cuh).  The others -- BN = 256, whose 128
+// accumulator registers per thread do not fit the 128 a 512-thread CTA allows, and the fp32 variant F = 2 -- keep the
+// whole epilogue on warpgroups 1-2.
 #include "gemm_epilogue.cuh"
 
 namespace {
@@ -38,18 +41,24 @@ struct IgemmParams {
   int bnr_C;
 };
 
-constexpr int kThreads = 384;           // producer warpgroup + two consumer warpgroups
 constexpr uint32_t kABytes = 128 * 128;  // one A stage: 128 rows x 64 bf16
-constexpr int kProducerRegs = 56, kConsumerRegs = 224;
+constexpr int kProducerRegs = 56, kConsumerRegs = 224;  // unstaged variants (384 threads): 128 * 56 + 256 * 224 <= 65536
 
-template <int BN>
+template <int BN, int F>
 struct Cfg {
+  static constexpr bool kStaged = F != 2 && BN <= 192;
+  static constexpr int kThreads = kStaged ? 512 : 384;  // + the store warpgroup
   static constexpr uint32_t kBBytes = BN * 128;
   static constexpr int kTbl = 128 * 9;  // ints of the per-tile index table [tap][row]
   static constexpr int kFixed = 1024 + kTbl * 4 + 256 + (2 * pnx::kEpiWarps + 5) * BN * 4;
-  static constexpr int kStagesRaw = (227 * 1024 - kFixed) / (int)(kABytes + kBBytes);
+  static constexpr int kStageBytes = (int)(kABytes + kBBytes);
+  static constexpr int kAvail = 227 * 1024 - kFixed;
+  // staged epilogue: the whole tile at once, or in two column halves where that would leave fewer than 3 stages
+  static constexpr int kPasses = !kStaged ? 1 : ((kAvail - pnx::Staging<BN, 1>::kBytes) / kStageBytes >= 3 ? 1 : 2);
+  static constexpr int kStgBytes = !kStaged ? 0 : pnx::Staging<BN, kPasses>::kBytes;
+  static constexpr int kStagesRaw = (kAvail - kStgBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr size_t kSmem = (size_t)kFixed + (size_t)kStages * (kABytes + kBBytes);
+  static constexpr size_t kSmem = (size_t)kFixed + (size_t)kStgBytes + (size_t)kStages * kStageBytes;
   static_assert(kStages >= 3, "pipeline depth");
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
@@ -59,9 +68,10 @@ __device__ __forceinline__ void named_bar_sync(int id, int n) {
 }
 
 template <int BN, int F>
-__global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constant__ CUtensorMap wmap, IgemmParams p) {
-  using C = Cfg<BN>;
+__global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __grid_constant__ CUtensorMap wmap, IgemmParams p) {
+  using C = Cfg<BN, F>;
   constexpr int kStages = C::kStages;
+  constexpr int kPasses = C::kPasses;
   constexpr uint32_t kBBytes = C::kBBytes;
   constexpr int kTbl = C::kTbl;
 
@@ -69,9 +79,12 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + (size_t)kStages * kABytes;
-  int* s_idx = reinterpret_cast<int*>(sB + (size_t)kStages * kBBytes);  // [T][128 rows] gathered row index, -1 = absent
+  uint8_t* stg = sB + (size_t)kStages * kBBytes;                        // staged output tile (pnx::Staging)
+  int* s_idx = reinterpret_cast<int*>(stg + C::kStgBytes);              // [T][128 rows] gathered row index, -1 = absent
   uint64_t* full = reinterpret_cast<uint64_t*>(s_idx + kTbl);
   uint64_t* empty = full + kStages;
+  uint64_t* staged = empty + kStages;  // the consumers' 256 threads wrote a staging pass
+  uint64_t* sfree = staged + 1;        // the store warpgroup has drained it
   float* s_stat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);  // [8 warps][2][BN] per-channel sums
   float* s_bias = s_stat + pnx::kEpiWarps * 2 * BN;                                  // [BN] bias of this CTA's columns
   float* s_bnc = s_bias + BN;                                                        // [4][BN] fused BN-backward affine
@@ -86,6 +99,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
       pnx::mbar_init(&full[s], 1 + 128);  // weight TMA (expect_tx) + the 128 gathering threads (cp.async arrive)
       pnx::mbar_init(&empty[s], 8);       // one arrival per consumer warp
     }
+    pnx::mbar_init(staged, 256);
+    pnx::mbar_init(sfree, 128);
     pnx::fence_barrier_init();
   }
   if (p.bias)
@@ -102,9 +117,22 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
   const int kpt = p.Cin >> 6;
   const int num_k = p.T * kpt * p.nseg;
 
-  if (wg == 0) {
+  if (wg == 3) {
+    // ---------------------------------------------------------------- store warpgroup (staged variants): drains the tiles
+    if constexpr (C::kStaged) {
+      const int stid = threadIdx.x - 384;
+      uint32_t spass = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const long long row0 = (long long)tile * 128;
+        pnx::gemm_epilogue_drain<BN, F, kPasses>(p.epi, row0, (int)min((long long)128, (long long)p.M - row0), n0, stg, s_stat,
+                                                 s_bnc, staged, sfree, spass, stid, 128, 2);
+      }
+      named_bar_sync(2, 128);
+      pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, stid, 128);
+    }
+  } else if (wg == 0) {
     // ---------------------------------------------------------------- producer
-    pnx::regs_dealloc<kProducerRegs>();
+    if constexpr (!C::kStaged) pnx::regs_dealloc<kProducerRegs>();
     const int ptid = threadIdx.x;
     const int sub = ptid & 7, rsub = ptid >> 3;  // a warp instruction copies 4 whole 128-byte rows
     const int hw = p.Hout * p.Wout;
@@ -162,7 +190,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
     }
   } else {
     // ---------------------------------------------------------------- consumers: wgmma + epilogue
-    pnx::regs_alloc<kConsumerRegs>();
+    if constexpr (!C::kStaged) pnx::regs_alloc<kConsumerRegs>();
+    uint32_t spass = 0;
     const int half = wg - 1;  // rows [64 * half, 64 * half + 64) of every tile
     int stage = 0;
     uint32_t phase = 0;
@@ -192,10 +221,16 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
       pnx::fence_acc(acc);
       if (lane == 0) pnx::mbar_arrive(&empty[prev]);
       const long long row0 = (long long)tile * 128;
-      pnx::gemm_epilogue<BN, F>(acc, p.epi, row0, (int)min((long long)128, (long long)p.M - row0), half, n0, s_bias, s_stat, s_bnc);
+      const int nvalid = (int)min((long long)128, (long long)p.M - row0);
+      if constexpr (C::kStaged)
+        pnx::gemm_epilogue_stage<BN, kPasses>(acc, p.epi, row0, nvalid, half, n0, s_bias, stg, staged, sfree, spass);
+      else
+        pnx::gemm_epilogue<BN, F>(acc, p.epi, row0, nvalid, half, n0, s_bias, s_stat, s_bnc);
     }
-    named_bar_sync(2, 256);
-    pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, threadIdx.x - 128, 256);
+    if constexpr (!C::kStaged) {
+      named_bar_sync(2, 256);
+      pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, threadIdx.x - 128, 256);
+    }
   }
 }
 
@@ -203,7 +238,7 @@ template <int BN, int F>
 int launch_igemm_f(const CUtensorMap& wmap, const IgemmParams& p, int n_blocks, int sm_count, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    PNX_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN>::kSmem));
+    PNX_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<BN, F>::kSmem));
     attr_set = true;
   }
   const int num_tiles = (p.M + 127) / 128;
@@ -211,7 +246,7 @@ int launch_igemm_f(const CUtensorMap& wmap, const IgemmParams& p, int n_blocks, 
   if (gx < 1) gx = 1;
   if (gx > num_tiles) gx = num_tiles;
   dim3 grid(gx, n_blocks);
-  igemm_kernel<BN, F><<<grid, kThreads, Cfg<BN>::kSmem, stream>>>(wmap, p);
+  igemm_kernel<BN, F><<<grid, Cfg<BN, F>::kThreads, Cfg<BN, F>::kSmem, stream>>>(wmap, p);
   PNX_CHECK_LAUNCH();
   return PNX_OK;
 }

@@ -8,8 +8,9 @@
 // 128B-swizzled smem buffer.  The three horizontal taps s = 0,1,2 are the SAME buffer read through wgmma descriptors
 // whose start address is shifted by s rows (s*128 bytes): 3 window loads feed 9 taps,
 // cutting the activation traffic 2.9x, and there are no gather warps at all (one thread issues every load).
-//   warpgroup 0: TMA producer (A windows, 4-D map [C, W, H, B]; weight tiles, 2-D map)
-//   warpgroups 1-2: wgmma on 64 pixels each, fp32 register accumulators, epilogue (gemm_epilogue.cuh)
+//   warpgroup 0: warp 0 is the TMA producer (A windows, 4-D map [C, W, H, B]; weight tiles, 2-D map), warps 1-3 store
+//                the staged output tiles and sum their statistics while the next tile's MMAs run (gemm_epilogue.cuh)
+//   warpgroups 1-2: wgmma on 64 pixels each, fp32 register accumulators, bias/ReLU/bf16 rounding into the staging buffer
 #include "gemm_epilogue.cuh"
 
 extern int g_pnx_deterministic;  // igemm.cu (pnx_set_deterministic)
@@ -41,9 +42,16 @@ struct WCfgWin {
   static constexpr uint32_t kWBytes = WS ? 9 * kBTap : 0;
   static constexpr uint32_t kStageBytes = WS ? kWinSlot : kWinSlot + 3 * kBTap;
   static constexpr int kFixed = 1024 + 256 + (2 * pnx::kEpiWarps + 5) * BN * 4;
-  static constexpr int kStagesRaw = (227 * 1024 - kFixed - (int)kWBytes) / (int)kStageBytes;
+  static constexpr int kAvail = 227 * 1024 - kFixed - (int)kWBytes;
+  // staged epilogue: the whole tile at once, or in two column halves where that would cost pipeline depth below 3 stages
+  // (or below what the ring had without staging, if that was less)
+  static constexpr int kStagesUnstaged = kAvail / (int)kStageBytes;
+  static constexpr int kMinStages = kStagesUnstaged < 3 ? kStagesUnstaged : 3;
+  static constexpr int kPasses = (kAvail - pnx::Staging<BN, 1>::kBytes) / (int)kStageBytes >= kMinStages ? 1 : 2;
+  static constexpr int kStgBytes = pnx::Staging<BN, kPasses>::kBytes;
+  static constexpr int kStagesRaw = (kAvail - kStgBytes) / (int)kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr size_t kSmem = kFixed + kWBytes + (size_t)kStages * kStageBytes;
+  static constexpr size_t kSmem = kFixed + kWBytes + (size_t)kStgBytes + (size_t)kStages * kStageBytes;
   static_assert(kStages >= 2, "stages");
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
@@ -65,12 +73,16 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_con
                                                                 const __grid_constant__ CUtensorMap wmap, WinParams p) {
   using C = WCfgWin<BN, WS>;
   constexpr int kStages = C::kStages;
+  constexpr int kPasses = C::kPasses;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem_w = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem = smem_w + C::kWBytes;  // stage ring (the stationary weight tiles, if any, come first)
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)kStages * C::kStageBytes);
+  uint8_t* stg = smem + (size_t)kStages * C::kStageBytes;  // staged output tile (pnx::Staging)
+  uint64_t* full = reinterpret_cast<uint64_t*>(stg + C::kStgBytes);
   uint64_t* empty = full + kStages;
   uint64_t* wfull = empty + kStages;
+  uint64_t* staged = wfull + 1;  // the consumers' 256 threads wrote a staging pass
+  uint64_t* sfree = staged + 1;  // the 96 store threads have drained it
   float* s_stat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);  // [8 warps][2][BN] per-channel sums
   float* s_bias = s_stat + pnx::kEpiWarps * 2 * BN;
   float* s_bnc = s_bias + BN;   // [4][BN] fused BN-backward: scale, shift, mean, invstd of this CTA's columns
@@ -85,6 +97,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_con
       pnx::mbar_init(&empty[s], 8);  // one arrival per consumer warp
     }
     pnx::mbar_init(wfull, 1);
+    pnx::mbar_init(staged, 256);
+    pnx::mbar_init(sfree, 96);
     pnx::fence_barrier_init();
   }
   if (p.bias)
@@ -101,8 +115,20 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_con
   const int kcc = p.Cin >> 6;
 
   if (wg == 0) {
-    pnx::regs_dealloc<40>();
-    if (threadIdx.x == 0) {
+    pnx::regs_dealloc<72>();  // gemm_epilogue_drain must fit in 72 registers: check `ptxas -v` for spills after editing it
+    if (threadIdx.x >= 32) {
+      // ---------------------------------------------------------------- warps 1-3: drain the staged tiles
+      const int stid = threadIdx.x - 32;
+      uint32_t spass = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int xc = tile % p.XC, by = tile / p.XC;
+        const long long row0 = (long long)by * p.W + xc * 128;
+        pnx::gemm_epilogue_drain<BN, F, kPasses>(p.epi, row0, min(128, p.W - xc * 128), n0, stg, s_stat, s_bnc, staged, sfree,
+                                                 spass, stid, 96, 2);
+      }
+      asm volatile("bar.sync 2, 96;" ::: "memory");
+      pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, stid, 96);
+    } else if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       if (WS) {
@@ -127,8 +153,9 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_con
       }
     }
   } else {
-    pnx::regs_alloc<224>();
+    pnx::regs_alloc<216>();  // 128 * 72 + 256 * 216 <= 65536
     const int half = wg - 1;  // pixels [64 * half, 64 * half + 64) of every tile
+    uint32_t spass = 0;
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];
@@ -164,10 +191,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_con
       pnx::fence_acc(acc);
       if (lane == 0) pnx::mbar_arrive(&empty[prev]);
       const long long row0 = (long long)by * p.W + xc * 128;  // pixel index of tile row 0 (by = b*H + y)
-      pnx::gemm_epilogue<BN, F>(acc, p.epi, row0, min(128, p.W - xc * 128), half, n0, s_bias, s_stat, s_bnc);
+      pnx::gemm_epilogue_stage<BN, kPasses>(acc, p.epi, row0, min(128, p.W - xc * 128), half, n0, s_bias, stg, staged, sfree, spass);
     }
-    asm volatile("bar.sync 2, 256;" ::: "memory");
-    pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, threadIdx.x - 128, 256);
   }
 }
 
