@@ -363,6 +363,34 @@ int pnx_det_decode_host(const float* out, long long ld, int B, int H, int W, int
                         float vs_x, float vs_y, float pc_x, float pc_y, float score_thr, const float* range6,
                         const float* rect, long long m, float* box9, float* score, int* label);
 
+/* ---------------------------------------------------------------- double-flip test-time augmentation
+ * pnx_flip4_points: points [n, 6] (batch_idx, x, y, z, intensity, time) -> out [4n, 6]: copy k of point i at row k*n + i
+ * with batch index 4b + k; k = 1 negates y, k = 2 negates x, k = 3 both (exact).  The rows are not grouped by frame
+ * (voxelize them with pnx_voxelize, not pnx_voxelize_frames); within a frame the input order is kept.
+ * pnx_det_*_flip4: the F1 entry points above with the same arguments, on the head output of such a batch: `out` is
+ * [4B*H*W, ld] (frame 4b + k = copy k of frame b) and B counts the B merged frames.  Each merged pixel (y, x) reads copy
+ * 1 at (H-1-y, x), copy 2 at (y, W-1-x), copy 3 at (H-1-y, W-1-x), undoes the mirror (y: reg_y -> 1 - reg_y, sin -> -sin,
+ * vy -> -vy; x: reg_x -> 1 - reg_x, cos -> -cos, vx -> -vx) and merges every quantity as ((v0 + v1) + (v2 + v3)) * 0.25f:
+ * hm after the sigmoid (then the first maximum over classes), dim after exp, height / reg / rot / vel / iou raw.  keys,
+ * seg_count, masks and results are those of the merged frames ([B*H*W], [B*C], ...).  The host twin takes HOST memory. */
+int pnx_flip4_points(const float* points, int n, float* out, cudaStream_t stream);
+int pnx_det_keys_flip4(const float* out, long long ld, int B, int H, int W, int C, const int* offs, float osf,
+                       float vs_x, float vs_y, float pc_x, float pc_y, float score_thr, const float* range6,
+                       const float* rect, long long* keys, int* seg_count, cudaStream_t stream);
+int pnx_det_nms_flip4(const float* out, long long ld, int B, int H, int W, int C, const int* offs, float osf, float vs_x,
+                      float vs_y, float pc_x, float pc_y, float score_thr, const float* range6, const float* rect,
+                      const float* nms_thr, const long long* order, const int* seg_start, const int* seg_count,
+                      int pre_max, int post_max, unsigned long long* mask, int* keep, int* keep_count,
+                      cudaStream_t stream);
+int pnx_det_gather_flip4(const float* out, long long ld, int B, int H, int W, int C, const int* offs, float osf,
+                         float vs_x, float vs_y, float pc_x, float pc_y, float score_thr, const float* range6,
+                         const float* rect, const long long* order, const int* seg_start, const int* keep,
+                         const int* keep_count, int post_max, int label_offset, float* det_box, float* det_score,
+                         long long* det_label, cudaStream_t stream);
+int pnx_det_decode_flip4_host(const float* out, long long ld, int B, int H, int W, int C, const int* offs, float osf,
+                              float vs_x, float vs_y, float pc_x, float pc_y, float score_thr, const float* range6,
+                              const float* rect, long long m, float* box9, float* score, int* label);
+
 #ifdef __cplusplus
 }
 #endif

@@ -82,6 +82,12 @@ _SIGS = {
     "pnx_aligned_iou3d": [P, P, I, P, P],
     "pnx_aligned_iou3d_host": [P, P],
     "pnx_det_decode_host": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, L, P, P, P],
+    # double-flip test-time augmentation: point expansion + the F1 entry points on the 4B-frame head output
+    "pnx_flip4_points": [P, I, P, P],
+    "pnx_det_keys_flip4": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, P, P, P],
+    "pnx_det_nms_flip4": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, P, P, P, P, I, I, P, P, P, P],
+    "pnx_det_gather_flip4": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, P, P, P, P, I, I, P, P, P, P],
+    "pnx_det_decode_flip4_host": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, L, P, P, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong,

@@ -586,12 +586,13 @@ class CenterHead(nn.Module):
         out_size_factor (per task), voxel_size, pc_range, nms.{nms_iou_threshold (per task, per class),
         nms_pre_max_size, nms_post_max_size}.  Returns a list (one per frame) of dicts box3d_lidar [K, 9]
         (x, y, z, dx, dy, dz, vx, vy, yaw), scores [K], label_preds [K] (int64), token.  One host sync (the kept counts)."""
-        def get(cfg, name):
-            return cfg[name] if isinstance(cfg, dict) or hasattr(cfg, "keys") else getattr(cfg, name)
-
+        get = _cfg_get
         raws = [getattr(pd.get("hm"), "_pnx_raw", None) for pd in preds_dicts]
         if any(r is None for r in raws):
             raise NotImplementedError("predict needs the fused head output (PillarNeXt-B heads: reg/height/dim/rot/vel/hm)")
+        double_flip = bool(get(test_cfg, "double_flip", False))
+        if double_flip:
+            self._check_double_flip(raws, test_cfg)
         nms = get(test_cfg, "nms")
         pre_max, post_max = int(get(nms, "nms_pre_max_size")), int(get(nms, "nms_post_max_size"))
         thr_all = get(nms, "nms_iou_threshold")
@@ -602,21 +603,23 @@ class CenterHead(nn.Module):
         osf_all = get(test_cfg, "out_size_factor")
         tokens = example.get("token") if isinstance(example, dict) else None
         results, flag = [], 0
+        copies = 4 if double_flip else 1
+        B = raws[0]["B"] // copies
         for t, r in enumerate(raws):
             off = r["off"]
             offs = [off["reg"], off["height"], off["dim"], off["rot"], off["vel"], off["hm"], off.get("iou", -1)]
             rect = [float(v) for v in self.rectifier[t]]
-            results.append(ops.det_postprocess(r["out"], r["B"], r["H"], r["W"], r["C"], offs, float(osf_all[t]), vs, pr,
+            results.append(ops.det_postprocess(r["out"], B, r["H"], r["W"], r["C"], offs, float(osf_all[t]), vs, pr,
                                                float(get(test_cfg, "score_threshold")), pcr, rect,
-                                               [float(v) for v in thr_all[t]], pre_max, post_max, label_offset=flag))
+                                               [float(v) for v in thr_all[t]], pre_max, post_max, label_offset=flag,
+                                               double_flip=double_flip))
             flag += self.num_classes[t]
         counts = torch.cat([res[3] for res in results]).cpu().tolist()       # the one host synchronisation
-        B = raws[0]["B"]
         out, base = [], 0
         bases = []
         for r in raws:
             bases.append(base)
-            base += r["B"] * r["C"]
+            base += B * r["C"]
         for b in range(B):
             boxes, scores, labels = [], [], []
             for t, (r, res) in enumerate(zip(raws, results)):
@@ -627,6 +630,37 @@ class CenterHead(nn.Module):
             out.append(dict(box3d_lidar=torch.cat(boxes), scores=torch.cat(scores), label_preds=torch.cat(labels),
                             token=tokens[b] if tokens is not None and len(tokens) > b else None))
         return out
+
+    def _check_double_flip(self, raws, test_cfg):
+        """Double flip merges each pixel with its mirror images, which only land on pixels when the grid is mirror
+        symmetric about the origin and the head maps cover it exactly; raise ValueError naming what does not hold."""
+        pr = [float(v) for v in _cfg_get(test_cfg, "pc_range")]
+        if len(pr) < 6 and len(getattr(self, "pc_range", [])) >= 6:
+            pr = self.pc_range
+        if len(pr) < 6:
+            raise ValueError("double_flip needs the 6-value pc_range (x_min, y_min, z_min, x_max, y_max, z_max) in the "
+                             "post-processing config to check that the grid is mirror symmetric")
+        if pr[0] != -pr[3] or pr[1] != -pr[4]:
+            raise ValueError("double_flip needs a mirror-symmetric grid: pc_range[0] == -pc_range[3] and pc_range[1] == "
+                             "-pc_range[4], got %s" % (pr,))
+        vs = [float(v) for v in _cfg_get(test_cfg, "voxel_size")]
+        gx, gy = int(round((pr[3] - pr[0]) / vs[0])), int(round((pr[4] - pr[1]) / vs[1]))
+        for t, r in enumerate(raws):
+            osf = int(_cfg_get(test_cfg, "out_size_factor")[t])
+            if r["W"] * osf != gx or r["H"] * osf != gy:
+                raise ValueError("double_flip needs head maps of grid / out_size_factor: task %d has %d x %d maps, the grid "
+                                 "%d x %d with out_size_factor %d" % (t, r["H"], r["W"], gy, gx, osf))
+            if r["B"] % 4:
+                raise ValueError("double_flip needs the head output of 4 mirrored copies per frame (ops.flip4_points), got "
+                                 "%d frames" % r["B"])
+
+
+def _cfg_get(cfg, name, *default):
+    """cfg.name or cfg[name] (the post-processing config may be a mapping or an attribute namespace); `default` when
+    given and the key is absent."""
+    if isinstance(cfg, dict) or hasattr(cfg, "keys"):
+        return cfg.get(name, *default) if default else cfg[name]
+    return getattr(cfg, name, *default)
 
 
 # =========================================================================================== detector
@@ -651,11 +685,11 @@ class SingleStageDetector(nn.Module):
             x = self.neck(x)
         return x
 
-    def _forward(self, example):
+    def _forward(self, example, copies=1):
         points = example["points"]
         if hasattr(self.reader, "batch_size"):
             tok = example.get("token") if isinstance(example, dict) else None
-            self.reader.batch_size = len(tok) if tok is not None and len(tok) > 0 else None
+            self.reader.batch_size = copies * len(tok) if tok is not None and len(tok) > 0 else None
         x = self.extract_feat(points)
         return self.head(x)
 
@@ -695,7 +729,22 @@ class SingleStageDetector(nn.Module):
 
     @torch.no_grad()
     def validation_step(self, example):
-        preds = self._forward(example)
+        """Eval forward + predict -> {token: detections on the host}.  With `post_processing.double_flip` set, every
+        frame runs four times (as is, mirrored in y, in x, in both: ops.flip4_points on the device, frames 4b + k) and
+        predict merges the four head outputs of each frame before decoding; the result is still one entry per token."""
+        if self.post_processing is not None and _cfg_get(self.post_processing, "double_flip", False):
+            flipped = dict(example)
+            flipped["points"] = ops.flip4_points(example["points"].float())
+            sorted_before = getattr(self.reader, "frame_sorted", None)
+            if sorted_before is not None:
+                self.reader.frame_sorted = False        # flip4_points writes copy k of the batch after copy k - 1
+            try:
+                preds = self._forward(flipped, copies=4)
+            finally:
+                if sorted_before is not None:
+                    self.reader.frame_sorted = sorted_before
+        else:
+            preds = self._forward(example)
         outputs = self.head.predict(example, preds, self.post_processing)
         detections = {}
         for output in outputs:

@@ -763,14 +763,17 @@ def _host_floats(vals, n):
 
 
 def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr, post_center_range, rectifier, nms_thr,
-                    pre_max, post_max, label_offset=0):
+                    pre_max, post_max, label_offset=0, double_flip=False):
     """One task of CenterHead.predict (centerhead.py:231-384): `out` = channels-last head output [B*H*W, ld] fp32,
     offs = column offsets (reg, height, dim, rot, vel, hm, iou or -1).  Returns det_box [B*C, post_max, 9], det_score
     [B*C, post_max], det_label [B*C, post_max] (int64, + label_offset) and keep_count [B*C] -- all on the device, no
     host synchronisation.  Segment s = frame * C + class.  The candidate ordering is one device sort (torch.sort of
-    the 64-bit keys the decode kernel builds); decode, IoU mask, greedy sweep and gather are libpnx kernels."""
+    the 64-bit keys the decode kernel builds); decode, IoU mask, greedy sweep and gather are libpnx kernels.
+    double_flip=True: `out` is the head output of a flip4_points batch, [4B*H*W, ld] (frame 4b + k = copy k of frame b);
+    the decode merges the four copies of each pixel (pnx_det_*_flip4, include/pnx.h) and the results are those of the
+    B original frames."""
     import ctypes
-    assert out.dtype == torch.float32 and out.is_cuda and out.dim() == 2 and out.shape[0] == B * H * W
+    assert out.dtype == torch.float32 and out.is_cuda and out.dim() == 2 and out.shape[0] == (4 if double_flip else 1) * B * H * W
     dev = out.device
     M, nseg = B * H * W, B * C
     offs_a = (ctypes.c_int * 7)(*[int(o) for o in offs])
@@ -782,8 +785,10 @@ def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr,
     keys = torch.empty(M, dtype=torch.int64, device=dev)
     seg_count = torch.empty(nseg, dtype=torch.int32, device=dev)
     L = lib()
+    keys_fn, nms_fn, gather_fn = ((L.pnx_det_keys_flip4, L.pnx_det_nms_flip4, L.pnx_det_gather_flip4) if double_flip else
+                                  (L.pnx_det_keys, L.pnx_det_nms, L.pnx_det_gather))
     _count(1)
-    check(L.pnx_det_keys(*common, ptr(keys), ptr(seg_count), stream()))
+    check(keys_fn(*common, ptr(keys), ptr(seg_count), stream()))
     order = torch.sort(keys)[1]
     seg_start = (torch.cumsum(seg_count, 0, dtype=torch.int32) - seg_count).contiguous()
     col_blocks = (pre_max + 63) // 64
@@ -791,15 +796,28 @@ def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr,
     keep = torch.empty(nseg * post_max, dtype=torch.int32, device=dev)
     keep_count = torch.empty(nseg, dtype=torch.int32, device=dev)
     _count(2)
-    check(L.pnx_det_nms(*common, ntp, ptr(order), ptr(seg_start), ptr(seg_count), int(pre_max), int(post_max), ptr(mask),
+    check(nms_fn(*common, ntp, ptr(order), ptr(seg_start), ptr(seg_count), int(pre_max), int(post_max), ptr(mask),
                         ptr(keep), ptr(keep_count), stream()))
     det_box = torch.empty(nseg, post_max, 9, dtype=torch.float32, device=dev)
     det_score = torch.empty(nseg, post_max, dtype=torch.float32, device=dev)
     det_label = torch.empty(nseg, post_max, dtype=torch.int64, device=dev)
     _count(1)
-    check(L.pnx_det_gather(*common, ptr(order), ptr(seg_start), ptr(keep), ptr(keep_count), int(post_max), int(label_offset),
-                           ptr(det_box), ptr(det_score), ptr(det_label), stream()))
+    check(gather_fn(*common, ptr(order), ptr(seg_start), ptr(keep), ptr(keep_count), int(post_max), int(label_offset),
+                    ptr(det_box), ptr(det_score), ptr(det_label), stream()))
     return det_box, det_score, det_label, keep_count
+
+
+def flip4_points(points):
+    """Double-flip test-time augmentation: points [N, 6] (b, x, y, z, i, t) fp32 cuda -> [4N, 6], copy k of point i at row
+    k*N + i in frame 4b + k (k = 1: y -> -y, k = 2: x -> -x, k = 3: both; pnx_flip4_points).  The rows are NOT grouped by
+    frame: voxelize them with frame_sorted=False."""
+    assert points.is_cuda and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 6, \
+        "points must be a CUDA float32 [N, 6] tensor (batch_idx, x, y, z, intensity, time)"
+    points = points.contiguous()
+    out = torch.empty(4 * points.shape[0], 6, dtype=torch.float32, device=points.device)
+    _count(1)
+    check(lib().pnx_flip4_points(ptr(points), points.shape[0], ptr(out), stream()))
+    return out
 
 
 def aligned_iou3d(boxes_a, boxes_b):
