@@ -391,6 +391,21 @@ int pnx_det_decode_flip4_host(const float* out, long long ld, int B, int H, int 
                               float vs_x, float vs_y, float pc_x, float pc_y, float score_thr, const float* range6,
                               const float* rect, long long m, float* box9, float* score, int* label);
 
+/* ---------------------------------------------------------------- global training augmentation
+ * pnx_global_aug: points [n, 6] (batch_idx, x, y, z, intensity, time) and raw boxes [B, M, 9] (x, y, z, dx, dy, dz, vx,
+ * vy, yaw) fp32 -> points_out, boxes_out (same shapes, new memory; the inputs are not written).  aug [B, 4, 4] fp64 holds
+ * per frame up to four records (code, p0, p1, p2), applied in slot order:
+ *   0 empty | 1 rotation (theta, cos theta, sin theta) | 2 scaling (s) | 3 translation (t, added to x, y and z) |
+ *   4 flip (fx, fy: nonzero = x flip (y -> -y), y flip (x -> -x)); other codes are no-ops.
+ * The results are those of the reference's numpy transforms (det3d/datasets/pipelines/augmentation.py +
+ * box_np_ops.rotate / scaling / translate / flip) to the bit, NaN box elements included (csrc/augment.cu lists the
+ * rounding rules).  One launch over n + B*M threads; the point order is kept.  A point whose batch index is not an
+ * integer in [0, B) is copied unchanged.  The host twin takes HOST memory. */
+int pnx_global_aug(const float* points, int n, const float* boxes, int B, int M, const double* aug, float* points_out,
+                   float* boxes_out, cudaStream_t stream);
+int pnx_global_aug_host(const float* points, int n, const float* boxes, int B, int M, const double* aug,
+                        float* points_out, float* boxes_out);
+
 #ifdef __cplusplus
 }
 #endif

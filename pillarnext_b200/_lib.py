@@ -88,6 +88,9 @@ _SIGS = {
     "pnx_det_nms_flip4": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, P, P, P, P, I, I, P, P, P, P],
     "pnx_det_gather_flip4": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, P, P, P, P, I, I, P, P, P, P],
     "pnx_det_decode_flip4_host": [P, L, I, I, I, I, P, F, F, F, F, F, F, P, P, L, P, P, P],
+    # global training augmentation (rotation, scaling, translation, flip) of points and raw boxes
+    "pnx_global_aug": [P, I, P, I, I, P, P, P, P],
+    "pnx_global_aug_host": [P, I, P, I, I, P, P, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong,

@@ -712,7 +712,21 @@ class SingleStageDetector(nn.Module):
         out.update(lab)
         return out
 
+    def global_aug(self, example):
+        """The frame-level training augmentation on the GPU: `aug` [B, 4, 4] fp64 (the records of det3d.datasets.
+        pipelines.augmentation, collated) is applied to `points` and `gt_boxes_raw` by ops.global_aug -- what the
+        reference's data-loader workers do in numpy before AssignLabel.  Returns the example without `aug`."""
+        if "hm" in example:
+            raise ValueError("the example already carries assigned labels (hm); the augmentation (aug) must be applied to "
+                             "the raw boxes before label assignment")
+        points, boxes = ops.global_aug(example["points"], example["gt_boxes_raw"], example["aug"])
+        out = {k: v for k, v in example.items() if k != "aug"}
+        out["points"], out["gt_boxes_raw"] = points, boxes
+        return out
+
     def training_step(self, example):
+        if "aug" in example:
+            example = self.global_aug(example)
         if "hm" not in example and "gt_boxes_raw" in example:
             example = self.assign_labels(example)
         if torch.is_grad_enabled():

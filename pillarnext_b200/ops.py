@@ -820,6 +820,26 @@ def flip4_points(points):
     return out
 
 
+def global_aug(points, gt_boxes, aug):
+    """Global training augmentation on the GPU (pnx_global_aug, include/pnx.h): points [N, 6] (b, x, y, z, i, t) fp32
+    cuda, raw boxes [B, M, 9] fp32 cuda and the collated records aug [B, 4, 4] fp64 cuda (det3d.datasets.pipelines.
+    augmentation) -> (points, boxes), new tensors with the reference's numpy results to the bit.  The inputs are left
+    untouched and the point order is kept, so frame-sorted points stay frame-sorted."""
+    assert points.is_cuda and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 6, \
+        "points must be a CUDA float32 [N, 6] tensor (batch_idx, x, y, z, intensity, time)"
+    assert gt_boxes.is_cuda and gt_boxes.dtype == torch.float32 and gt_boxes.dim() == 3 and gt_boxes.shape[2] == 9, \
+        "gt_boxes must be a CUDA float32 [B, M, 9] tensor"
+    assert aug.is_cuda and aug.dtype == torch.float64 and tuple(aug.shape) == (gt_boxes.shape[0], 4, 4), \
+        "aug must be a CUDA float64 [B, 4, 4] tensor (B = gt_boxes.shape[0])"
+    points, gt_boxes, aug = points.contiguous(), gt_boxes.contiguous(), aug.contiguous()
+    pts_out, box_out = torch.empty_like(points), torch.empty_like(gt_boxes)
+    B, M = gt_boxes.shape[:2]
+    _count(1)
+    check(lib().pnx_global_aug(ptr(points), points.shape[0], ptr(gt_boxes), B, M, ptr(aug), ptr(pts_out), ptr(box_out),
+                               stream()))
+    return pts_out, box_out
+
+
 def aligned_iou3d(boxes_a, boxes_b):
     """[n, 7] x [n, 7] fp32 (x, y, z, dx, dy, dz, heading) -> [n] aligned 3-D IoU (iou3d_nms_utils.py:45-87)."""
     assert boxes_a.shape == boxes_b.shape and boxes_a.shape[-1] == 7 and boxes_a.is_cuda

@@ -8,11 +8,13 @@ under a box are removed).  Class-dependent sizes make the classes separable.
 
 SyntheticSceneDataset follows det3d/datasets/base.py (`__len__`, `__getitem__`, `evaluation(detections, output_dir)`,
 base.py:48-108) as far as the hot path needs it; label assignment is NOT done on the CPU workers (assign.py) -- the
-collated batch carries the raw boxes and the detector builds the targets on the GPU (pnx_assign_labels, row F3)."""
+collated batch carries the raw boxes and the detector builds the targets on the GPU (pnx_assign_labels, row F3).
+Global augmentation (`augmentation=`, base.py:97-99) is split the same way: the drop-in transforms of
+det3d.datasets.pipelines.augmentation draw their parameters here and the detector applies them on the GPU."""
 import numpy as np
 import torch
 
-from . import synth
+from . import hydra_lite, synth
 
 # nominal (dx, dy, dz) per class, metres (nuScenes / Waymo class vocabulary of the reference configs)
 CLASS_SIZES = {
@@ -95,12 +97,19 @@ def make_scene(seed, cfg, n_points=6000, n_boxes=12):
 
 class SyntheticSceneDataset(torch.utils.data.Dataset):
     """Frames are generated on the fly from (seed0 + index): an unbounded, reproducible stream; train and held-out
-    splits are disjoint seed ranges."""
+    splits are disjoint seed ranges.
 
-    def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None, **_):
+    augmentation: dict of `_target_` nodes (or transform objects) applied to every frame in dict order after the scene
+    is made, as the reference's BaseDataset does; each appends its record to the frame's `aug` list."""
+
+    def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
+                 augmentation=None, **_):
         self.cfg, self.n_frames, self.seed0, self.n_points, self.n_boxes = cfg, int(n_frames), int(seed0), int(n_points), int(n_boxes)
         self.test_mode = test_mode
         self.class_names = [n for t in cfg["tasks"] for n in t]
+        if augmentation and test_mode:
+            raise ValueError("augmentation is a training transform: a test_mode dataset must not set it")
+        self.augmentations = hydra_lite.instantiate(augmentation) if augmentation else None
 
     def __len__(self):
         return self.n_frames
@@ -108,7 +117,11 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     def __getitem__(self, i):
         pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
         cls = np.array([self.class_names.index(n) for n in names], dtype=np.int32)
-        return {"points": pts, "gt_boxes_raw": boxes, "gt_classes": cls, "token": "scene_%d" % (self.seed0 + i)}
+        res = {"points": pts, "gt_boxes_raw": boxes, "gt_classes": cls, "token": "scene_%d" % (self.seed0 + i)}
+        if self.augmentations is not None:
+            for aug in self.augmentations.values():
+                res = aug(res)
+        return res
 
     def ground_truth(self):
         gts = {}
@@ -125,7 +138,8 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
 
 def collate(batch_list):
     """loader/collate.py:6-35 for this dataset: points get the frame index prepended; raw boxes are padded to the
-    longest frame (class -1 = padding)."""
+    longest frame (class -1 = padding).  Frames with augmentation records add aug [B, 4, 4] float64: frame i's records
+    (code, p0, p1, p2) in slots 0.., the rest zero (empty)."""
     pts = [np.pad(b["points"], ((0, 0), (1, 0)), mode="constant", constant_values=i) for i, b in enumerate(batch_list)]
     m = max(1, max(len(b["gt_classes"]) for b in batch_list))
     boxes = np.zeros((len(batch_list), m, 9), dtype=np.float32)
@@ -135,5 +149,15 @@ def collate(batch_list):
         k = len(b["gt_classes"])
         boxes[i, :k] = b["gt_boxes_raw"]
         cls[i, :k] = b["gt_classes"]
-    return {"points": torch.tensor(np.concatenate(pts, 0)), "gt_boxes_raw": torch.tensor(boxes), "gt_classes": torch.tensor(cls),
-            "token": [b["token"] for b in batch_list]}
+    out = {"points": torch.tensor(np.concatenate(pts, 0)), "gt_boxes_raw": torch.tensor(boxes), "gt_classes": torch.tensor(cls),
+           "token": [b["token"] for b in batch_list]}
+    if any("aug" in b for b in batch_list):
+        aug = np.zeros((len(batch_list), 4, 4), dtype=np.float64)
+        for i, b in enumerate(batch_list):
+            rec = b.get("aug", [])
+            if len(rec) > 4:
+                raise ValueError("at most 4 augmentation records per frame, got %d" % len(rec))
+            if rec:
+                aug[i, :len(rec)] = rec
+        out["aug"] = torch.tensor(aug)
+    return out
