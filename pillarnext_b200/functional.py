@@ -515,12 +515,17 @@ class BNActFn(torch.autograd.Function):
         assert dy.shape[1] == P * C
         ysrc = y if ctx.has_res else None
         red = ops.bn_bwd_reduce_split(dy, C, ysrc, C, x_raw, M, C, mean, invstd, ctx.relu, (scale, shift))
-        local = red
+        local, count = red, ctx.count
         if ctx.sync:
-            raise NotImplementedError("SyncBatchNorm backward is not available in the fp32-grade split mode (single-GPU parity tool)")
+            # SyncBatchNorm: the two sums over all ranks (dgamma / dbeta stay local, DDP averages them).  The split apply
+            # kernel takes a host count, so the global population is read from the device here: one synchronisation per
+            # BatchNorm, acceptable in this verification mode (the bf16 path passes the device count instead)
+            red = local.clone()
+            dist.all_reduce(red)
+            count = int(ctx.count_dev.item())
         dxs = torch.empty(M, P * C, dtype=torch.bfloat16, device=dy.device)
         dres = torch.empty(M, P * C, dtype=torch.bfloat16, device=dy.device) if ctx.has_res else None
-        ops.bn_bwd_apply_split(dy, C, ysrc, C, x_raw, M, C, mean, invstd, gamma, red, ctx.count, ctx.relu, (scale, shift),
+        ops.bn_bwd_apply_split(dy, C, ysrc, C, x_raw, M, C, mean, invstd, gamma, red, count, ctx.relu, (scale, shift),
                                dxs, C, dres=dres, dres_lo=C)
         dx = ops.rows_merge(dxs, C, C)          # x_raw is an fp32 [M, C] tensor: its gradient has the same shape / dtype
         r = local.float()
