@@ -56,14 +56,6 @@ struct WCfgWin {
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
 
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
-          "r"(pnx::smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(pnx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 __device__ __forceinline__ uint64_t desc_sw128_off(uint32_t addr, uint32_t base_off) {
   return pnx::make_smem_desc_sw128(addr, 16, 1024) | ((uint64_t)(base_off & 7u) << 49);
 }
@@ -143,7 +135,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_win_kernel(const __grid_con
             pnx::mbar_wait(&empty[stage], phase ^ 1);
             uint8_t* st = smem + (size_t)stage * C::kStageBytes;
             pnx::mbar_arrive_expect_tx(&full[stage], WS ? kWinBytes : kWinBytes + 3 * C::kBTap);
-            tma_load_4d(&amap, &full[stage], st, cc * 64, xc * 128 - 1, y + r - 1, b);
+            pnx::tma_load_4d(&amap, &full[stage], st, cc * 64, xc * 128 - 1, y + r - 1, b);
 #pragma unroll
             for (int s = 0; s < 3; ++s)
               if (!WS) pnx::tma_load_2d(&wmap, &full[stage], st + kWinSlot + s * C::kBTap, cc * 64, (r * 3 + s) * p.Cout_total + n0);
@@ -221,9 +213,6 @@ int launch_win(const CUtensorMap& amap, const CUtensorMap& wmap, const WinParams
 }
 
 }  // namespace
-
-int pnx_encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3],
-                            const uint32_t box[4]);
 
 // Contract: include/pnx.h (pnx_conv3x3_win).
 extern "C" int pnx_conv3x3_win(const void* A, long long lda, int B, int H, int W, int Cin, const void* Wpacked, int Cout,

@@ -110,6 +110,14 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// 4-D tiled load, coordinates innermost first; out-of-bounds elements (negative coordinates included) are zero-filled
+__device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
+          "r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 
 // ------------------------------------------------------------------ cp.async (gathered rows)
 // 16-byte global -> shared copy; src_bytes = 0 zero-fills the destination (absent neighbour / padding row)
@@ -171,3 +179,6 @@ __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(_
 // Resolved through cudaGetDriverEntryPoint so the library links without libcuda.
 int pnx_encode_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                             uint64_t row_stride_bytes, uint32_t box_rows, uint32_t box_cols);
+// host: 4-D bf16 tensor map, dims / box innermost first, strides of dims 1..3 in bytes, SWIZZLE_128B.
+int pnx_encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3],
+                            const uint32_t box[4]);

@@ -16,6 +16,17 @@
 // cp.async, each warp gathering the rows whose indices its lanes hold; warpgroups 1-2: wgmma, then a split's slab (or
 // red.global.add) from registers.  With a 64-channel X both consumer warpgroups multiply the one X block, each over
 // half of the group's columns.  Either way every dW element is one accumulator summing the split's rows in order.
+// Window producer (WIN; dense 3 x 3, stride 1, dilation 1, 'same', image width a multiple of 16; see igemm_win.cu for the
+// forward's version): a CTA's tap group is one kernel row r, and a K chunk is up to `chunk` consecutive pixels of one
+// image row inside one split.  Per chunk one thread issues the X tiles and ONE 4-D TMA load of the (chunk + 2)-pixel
+// window of Y at image row y + r - 1, zero-filled outside the image (the padding the gather path zero-fills per absent
+// neighbour).  Tap s of the row is the window shifted by s
+// pixels = s * 128 bytes, so the wgmma descriptor with LBO = 128 bytes reads the three taps as three side-by-side
+// 64-channel column blocks of the one buffer (the 128B swizzle is applied on absolute shared-memory address bits, as
+// igemm_win.cu relies on too): one window load feeds three taps, where the gather path copies each row once per tap.
+// Both paths run the same split plan and the same k16 steps (16 consecutive rows; with W % 16 == 0 they never straddle
+// an image row) in the same order; the X rows of a short chunk's unused k16 steps are zero-filled, so those steps add
+// exact zeros.  The window path's dW is therefore bit-identical to the gather path's.
 // This is the backward of: spconv SparseConv2d/SubMConv2d (reference sparse_conv.py:25-29,50-51),
 // nn.Conv2d/F.conv2d (aspp.py:19-32, conv.py:9-10, centerhead.py:35-46,108-114), nn.ConvTranspose2d
 // (centerhead.py:26-27) -- autograd derives these in the reference (trainer.py:94-108 loss.backward()).
@@ -38,20 +49,29 @@ struct WgradParams {
   int y_chunks;    // Y_total / NYC
   int taps_per_group;
   int rows_per_split;
+  int chunk;       // window path: most pixels per K chunk (16 * WKS)
 };
 
 constexpr int kThreads = 384;         // producer warpgroup + two consumer warpgroups
 constexpr int kKS = 64;               // rows (K) per stage
 constexpr uint32_t kBlk = kKS * 128;  // bytes of one [64 rows x 64 ch] block
+constexpr int kWinMaxChunk = 128;
+constexpr uint32_t kWinXAtom = kWinMaxChunk * 128;  // one [chunk pixels x 64 ch] X tile of the window path
+constexpr uint32_t kWinSlot = 17 * 1024;  // the (chunk + 2)-pixel window, plus the row a fourth shifted column block reads
 
 // NYC = Y channels per CTA (64..256), TG = taps per group: one MMA per k16 step spans the N = NYC * TG columns of the
 // group.  XD (X has 64 channels): both consumer warpgroups multiply the one X block, each over half of the columns.
-template <int NYC, int TG, bool XD>
+// WKS > 0: the window path (WIN), chunks of up to 16 * WKS pixels.  NYC = 64 and the group is one kernel row; with XD the
+// columns are four shifts of the window, two per warpgroup, and the fourth (shift 3) is computed and never stored, as the
+// padding taps of the gather path are.
+template <int NYC, int TG, bool XD, int WKS>
 struct WCfg {
+  static constexpr bool WIN = WKS > 0;
   static constexpr int kN = NYC * TG;
   static constexpr int kNW = XD ? kN / 2 : kN;  // accumulator columns of one consumer warpgroup
   static constexpr int kYAtoms = NYC / 64;
-  static constexpr uint32_t kStageBytes = (2 + TG * kYAtoms) * kBlk;
+  static constexpr uint32_t kXBytes = WIN ? (XD ? 1 : 2) * kWinXAtom : 2 * kBlk;  // the X tiles of a stage come first
+  static constexpr uint32_t kStageBytes = kXBytes + (WIN ? kWinSlot : TG * kYAtoms * kBlk);
   static constexpr int kStagesRaw = (200 * 1024) / (int)kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
   static constexpr size_t kSmem = 1024 + (size_t)kStages * kStageBytes + 256;
@@ -59,11 +79,27 @@ struct WCfg {
   static_assert(!XD || kN % 128 == 0, "a warpgroup's half of the columns is whole 64-channel atoms");
   static_assert(kStages >= 2, "need at least two stages");
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
+  static_assert(!WIN || (NYC == 64 && TG == (XD ? 4 : 3)), "window: the three taps of one kernel row, 64 Y channels");
+  static_assert((kWinMaxChunk + 2 + 1) * 128 <= kWinSlot, "window slot");
 };
 
-template <int NYC, int TG, bool XD>
-__global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constant__ CUtensorMap xmap, WgradParams p) {
-  using C = WCfg<NYC, TG, XD>;
+// window path: chunks of the split's rows [m_begin, m_end) -- image-row pieces, each cut into runs of at most `chunk`
+__device__ __forceinline__ int win_chunks(int m_begin, int m_end, int W, int chunk) {
+  int n = 0;
+  for (int m = m_begin; m < m_end;) {
+    const int e = min(m_end, (m / W + 1) * W);
+    n += (e - m + chunk - 1) / chunk;
+    m = e;
+  }
+  return n;
+}
+
+// xmap: X, 2-D [M, X_total] (gather path) or 4-D [X_total, W, H, B] (window path); ymap: Y, 4-D (window path only)
+template <int NYC, int TG, bool XD, int WKS>
+__global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constant__ CUtensorMap xmap,
+                                                            const __grid_constant__ CUtensorMap ymap, WgradParams p) {
+  using C = WCfg<NYC, TG, XD, WKS>;
+  constexpr bool WIN = C::WIN;
   constexpr int kStages = C::kStages, kYAtoms = C::kYAtoms, kNW = C::kNW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -73,21 +109,22 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constan
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int xb = blockIdx.x / p.y_chunks, yc = blockIdx.x - xb * p.y_chunks;
   const int t0 = blockIdx.y * p.taps_per_group;
-  const int ntaps = min(TG, p.T - t0);  // taps [ntaps, TG) of the group are zero tiles
+  const int ntaps = WIN ? 3 : min(TG, p.T - t0);  // taps [ntaps, TG) of the group are zero tiles (window: never stored)
   const int split = blockIdx.z;
   const int m_begin = split * p.rows_per_split;
   const int m_end = min(p.M, m_begin + p.rows_per_split);
-  const int num_k = (m_end - m_begin + kKS - 1) / kKS;
+  const int num_k = WIN ? win_chunks(m_begin, m_end, p.Wout, p.chunk) : (m_end - m_begin + kKS - 1) / kKS;
 
   if (threadIdx.x == 0) {
     pnx::tma_prefetch_desc(&xmap);
+    if (WIN) pnx::tma_prefetch_desc(&ymap);
     for (int s = 0; s < kStages; ++s) {
-      pnx::mbar_init(&full[s], 1 + 128);  // X tiles (expect_tx) + the 128 gathering threads (cp.async arrive)
-      pnx::mbar_init(&empty[s], 8);       // one arrival per consumer warp
+      pnx::mbar_init(&full[s], WIN ? 1 : 1 + 128);  // X tiles (expect_tx) + the 128 gathering threads (cp.async arrive)
+      pnx::mbar_init(&empty[s], 8);                 // one arrival per consumer warp
     }
     pnx::fence_barrier_init();
   }
-  if (ntaps < TG) {
+  if (!WIN && ntaps < TG) {
     // the Y tiles of the padding taps are zeroed once in every stage and never written again
     constexpr int kPer = kBlk / 16;  // 16-byte words of one block
     const int pad_words = (TG - ntaps) * kYAtoms * kPer;
@@ -100,8 +137,36 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constan
   __syncthreads();
   if (num_k <= 0) return;
 
-  if (wg == 0) {
-    // ---------------------------------------------------------------- producer
+  if (wg == 0 && WIN) {
+    // ---------------------------------------------------------------- producer, window path: one thread, TMA only
+    pnx::regs_dealloc<56>();
+    if (threadIdx.x == 0) {
+      const int r = blockIdx.y;  // kernel row of the group: taps 3r .. 3r+2
+      constexpr int nblk = XD ? 1 : 2;
+      const uint32_t tx = (uint32_t)(nblk * p.chunk + p.chunk + 2) * 128;
+      int stage = 0;
+      uint32_t phase = 0;
+      int m = m_begin;
+      for (int kc = 0; kc < num_k; ++kc) {
+        const int by = m / p.Wout, x0 = m - by * p.Wout;
+        const int len = min(min(m_end, (by + 1) * p.Wout) - m, p.chunk);  // a multiple of 16
+        const int y = by % p.Hout, b = by / p.Hout;
+        pnx::mbar_wait(&empty[stage], phase ^ 1);
+        uint8_t* st = smem + (size_t)stage * C::kStageBytes;
+        pnx::mbar_arrive_expect_tx(&full[stage], tx);
+        // X in 16-pixel boxes, one per k16 step; the steps past the chunk's length load a box wholly outside the image
+        // (x = W), i.e. zeros, and add nothing
+#pragma unroll
+        for (int i = 0; i < WKS; ++i)
+          for (int b2 = 0; b2 < nblk; ++b2)
+            pnx::tma_load_4d(&xmap, &full[stage], st + b2 * kWinXAtom + i * 2048, xb * 128 + b2 * 64, 16 * i < len ? x0 + 16 * i : p.Wout, y, b);
+        pnx::tma_load_4d(&ymap, &full[stage], st + C::kXBytes, yc * 64, x0 - 1, y + r - 1, b);
+        m += len;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else if (wg == 0) {
+    // ---------------------------------------------------------------- producer, gather path
     pnx::regs_dealloc<56>();
     const int warp = threadIdx.x >> 5;
     const int y_ch0 = yc * NYC;
@@ -176,8 +241,11 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constan
     // X channels [64 * half, +64) of the block over all columns, or (XD) the one X block over columns [kNW * half, +kNW)
     pnx::regs_alloc<224>();
     const int half = wg - 1;
-    const uint32_t x_off = XD ? 0u : (uint32_t)half * kBlk;
-    const uint32_t y_off = 2 * kBlk + (XD ? (uint32_t)half * (kNW / 64) * kBlk : 0u);
+    const uint32_t x_off = XD ? 0u : (uint32_t)half * (WIN ? kWinXAtom : kBlk);
+    // window: column block s of the B operand is the window shifted by s pixels (LBO = one 128-byte pixel row)
+    const uint32_t y_off = C::kXBytes + (XD ? (uint32_t)half * (kNW / 64) * (WIN ? 128u : kBlk) : 0u);
+    const uint32_t y_lbo = WIN ? 128u : kBlk;
+    constexpr int ksteps = WIN ? WKS : kKS / 16;
     float acc[kNW / 2];
 #pragma unroll
     for (int i = 0; i < kNW / 2; ++i) acc[i] = 0.f;
@@ -190,9 +258,9 @@ __global__ void __launch_bounds__(kThreads, 1) wgrad_kernel(const __grid_constan
       pnx::fence_acc(acc);
       const uint32_t st = pnx::smem_u32(smem + (size_t)stage * C::kStageBytes);
 #pragma unroll
-      for (int k = 0; k < kKS / 16; ++k)
+      for (int k = 0; k < ksteps; ++k)
         pnx::Wgmma<kNW, 1, 1>::mma(acc, pnx::make_smem_desc_sw128(st + x_off + k * 2048, kBlk, 1024),
-                                   pnx::make_smem_desc_sw128(st + y_off + k * 2048, kBlk, 1024), (kc > 0 || k > 0) ? 1u : 0u);
+                                   pnx::make_smem_desc_sw128(st + y_off + k * 2048, y_lbo, 1024), (kc > 0 || k > 0) ? 1u : 0u);
       pnx::wgmma_commit();
       pnx::wgmma_wait<1>();  // the previous stage's MMAs are done: release it
       if (kc > 0 && lane == 0) pnx::mbar_arrive(&empty[prev]);
@@ -267,19 +335,32 @@ inline WPlan wgrad_plan(int x_blocks, int Y_total, int T, int M, int sm_count) {
   return w;
 }
 
-template <int NYC, int TG, bool XD>
-int launch_wgrad(const CUtensorMap& xmap, WgradParams p, int x_blocks, int sm_count, cudaStream_t stream) {
+// Window path: most pixels per K chunk for an image row of W pixels.  The chunk is the multiple of 16 (one wgmma k-step)
+// in [64, 128] with the fewest zero k16 steps ceil(W / chunk) * chunk - W per whole row, the wider one on a tie (fewer
+// windows, and the two extra pixels of each window are a smaller share): 112 for W = 336 (none), 96 for 176.  Rows that a
+// split boundary cuts cost up to one more partial chunk each.
+inline int wgrad_win_chunk(int W) {
+  int best = kWinMaxChunk;
+  for (int c = kWinMaxChunk; c >= 64; c -= 16)
+    if ((W + c - 1) / c * c < (W + best - 1) / best * best) best = c;
+  return best;
+}
+
+template <int NYC, int TG, bool XD, int WKS>
+int launch_wgrad(const CUtensorMap& xmap, const CUtensorMap& ymap, WgradParams p, int x_blocks, int sm_count, cudaStream_t stream) {
+  using C = WCfg<NYC, TG, XD, WKS>;
+  constexpr bool WIN = C::WIN;
   static bool attr_set = false;
   if (!attr_set) {
-    PNX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NYC, TG, XD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WCfg<NYC, TG, XD>::kSmem));
+    PNX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NYC, TG, XD, WKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmem));
     attr_set = true;
   }
-  const WPlan w = wgrad_plan(x_blocks, p.Y_total, p.T, p.M, sm_count);
+  const WPlan w = wgrad_plan(x_blocks, p.Y_total, p.T, p.M, sm_count);  // the window path splits the rows as the gather path does
   p.y_chunks = p.Y_total / NYC;
-  p.taps_per_group = TG;
+  p.taps_per_group = WIN ? 3 : TG;
   p.rows_per_split = w.rows_per_split;
-  dim3 grid(x_blocks * p.y_chunks, (p.T + TG - 1) / TG, w.splits);
-  wgrad_kernel<NYC, TG, XD><<<grid, kThreads, WCfg<NYC, TG, XD>::kSmem, stream>>>(xmap, p);
+  dim3 grid(x_blocks * p.y_chunks, WIN ? 3 : (p.T + TG - 1) / TG, w.splits);
+  wgrad_kernel<NYC, TG, XD, WKS><<<grid, kThreads, C::kSmem, stream>>>(xmap, ymap, p);
   PNX_CHECK_LAUNCH();
   if (p.partials) {
     const long long n = (long long)p.T * p.X_total * p.Y_total;
@@ -287,6 +368,13 @@ int launch_wgrad(const CUtensorMap& xmap, WgradParams p, int x_blocks, int sm_co
     PNX_CHECK_LAUNCH();
   }
   return PNX_OK;
+}
+
+template <int WKS>
+int launch_wgrad_win(const CUtensorMap& xmap, const CUtensorMap& ymap, const WgradParams& p, int x_blocks, int sm_count,
+                     cudaStream_t stream) {
+  if (p.X_total == 64) return launch_wgrad<64, 4, true, WKS>(xmap, ymap, p, x_blocks, sm_count, stream);
+  return launch_wgrad<64, 3, false, WKS>(xmap, ymap, p, x_blocks, sm_count, stream);
 }
 
 }  // namespace
@@ -320,24 +408,54 @@ extern "C" int pnx_wgrad(const void* X, long long ldx, int x_channels, const voi
   p.dW = dW; p.partials = partials; p.X_total = x_channels; p.Y_total = y_channels;
   PNX_CHECK_ARG(!partials || (reinterpret_cast<uintptr_t>(partials) & 15) == 0, "partials 16-byte aligned");
   p.y_chunks = 1; p.taps_per_group = 1; p.rows_per_split = M;
+  p.chunk = 0;
   const int x_blocks = x_channels == 64 ? 1 : x_channels / 128;
   PNX_CHECK_ARG((reinterpret_cast<uintptr_t>(X) & 15) == 0 && (reinterpret_cast<uintptr_t>(Y) & 15) == 0, "X/Y 16-byte aligned");
+  PNX_CHECK_ARG(y_rows >= 1 && y_rows < 0x7fffffffLL, "y_rows = number of rows of Y");
+  const long long hw = (long long)p.Hout * p.Wout;
+  // W % 16 == 0: no k16 step of 16 consecutive rows straddles an image row, so the window path can run the gather path's
+  // k16 steps and sum every dW element in the same order
+  const bool window = gathered && !nbr && !shuffle && taps == 9 && kw == 3 && mul == 1 && dil == 1 && pad == 1 && Hin == p.Hout &&
+                      Win == p.Wout && p.Wout % 16 == 0 && M % hw == 0 && y_rows >= M;
+  if (window) {
+    const int B = (int)(M / hw);
+    p.chunk = wgrad_win_chunk(p.Wout);
+    CUtensorMap xmap, ymap;
+    const uint64_t xdims[4] = {(uint64_t)x_channels, (uint64_t)p.Wout, (uint64_t)p.Hout, (uint64_t)B};
+    const uint64_t xstr[3] = {(uint64_t)ldx * 2, (uint64_t)p.Wout * ldx * 2, (uint64_t)hw * ldx * 2};
+    const uint32_t xbox[4] = {64, 16, 1, 1};
+    int rc = pnx_encode_tmap_4d_bf16(&xmap, X, xdims, xstr, xbox);
+    if (rc) return rc;
+    const uint64_t ydims[4] = {(uint64_t)y_channels, (uint64_t)p.Wout, (uint64_t)p.Hout, (uint64_t)B};
+    const uint64_t ystr[3] = {(uint64_t)ldy * 2, (uint64_t)p.Wout * ldy * 2, (uint64_t)hw * ldy * 2};
+    const uint32_t ybox[4] = {64, (uint32_t)p.chunk + 2, 1, 1};
+    rc = pnx_encode_tmap_4d_bf16(&ymap, Y, ydims, ystr, ybox);
+    if (rc) return rc;
+    // the k-steps per chunk are a template argument: a run-time trip count around the MMAs would serialize them
+    switch (p.chunk / 16) {
+      case 4: return launch_wgrad_win<4>(xmap, ymap, p, x_blocks, sm_count, stream);
+      case 5: return launch_wgrad_win<5>(xmap, ymap, p, x_blocks, sm_count, stream);
+      case 6: return launch_wgrad_win<6>(xmap, ymap, p, x_blocks, sm_count, stream);
+      case 7: return launch_wgrad_win<7>(xmap, ymap, p, x_blocks, sm_count, stream);
+      default: return launch_wgrad_win<8>(xmap, ymap, p, x_blocks, sm_count, stream);
+    }
+  }
   CUtensorMap xmap;
   int rc = pnx_encode_tmap_2d_bf16(&xmap, X, (uint64_t)M, (uint64_t)x_channels, (uint64_t)ldx * 2, kKS, 64);
   if (rc) return rc;
-  PNX_CHECK_ARG(y_rows >= 1 && y_rows < 0x7fffffffLL, "y_rows = number of rows of Y");
+  const CUtensorMap& ymap = xmap;  // not read by the gather path
   int NYC, TG;
   if (x_channels == 64) {
     wgrad_variant(y_channels, taps, true, &NYC, &TG);
-    if (NYC == 256) return launch_wgrad<256, 1, true>(xmap, p, x_blocks, sm_count, stream);
-    if (NYC == 128) return TG == 2 ? launch_wgrad<128, 2, true>(xmap, p, x_blocks, sm_count, stream) : launch_wgrad<128, 1, true>(xmap, p, x_blocks, sm_count, stream);
-    return TG == 4 ? launch_wgrad<64, 4, true>(xmap, p, x_blocks, sm_count, stream) : launch_wgrad<64, 2, true>(xmap, p, x_blocks, sm_count, stream);
+    if (NYC == 256) return launch_wgrad<256, 1, true, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+    if (NYC == 128) return TG == 2 ? launch_wgrad<128, 2, true, 0>(xmap, ymap, p, x_blocks, sm_count, stream) : launch_wgrad<128, 1, true, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+    return TG == 4 ? launch_wgrad<64, 4, true, 0>(xmap, ymap, p, x_blocks, sm_count, stream) : launch_wgrad<64, 2, true, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
   }
   wgrad_variant(y_channels, taps, false, &NYC, &TG);
-  if (NYC == 256) return launch_wgrad<256, 1, false>(xmap, p, x_blocks, sm_count, stream);
-  if (NYC == 192) return launch_wgrad<192, 1, false>(xmap, p, x_blocks, sm_count, stream);
-  if (NYC == 128) return TG == 2 ? launch_wgrad<128, 2, false>(xmap, p, x_blocks, sm_count, stream) : launch_wgrad<128, 1, false>(xmap, p, x_blocks, sm_count, stream);
-  if (TG == 4) return launch_wgrad<64, 4, false>(xmap, p, x_blocks, sm_count, stream);
-  if (TG == 3) return launch_wgrad<64, 3, false>(xmap, p, x_blocks, sm_count, stream);
-  return launch_wgrad<64, 1, false>(xmap, p, x_blocks, sm_count, stream);
+  if (NYC == 256) return launch_wgrad<256, 1, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+  if (NYC == 192) return launch_wgrad<192, 1, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+  if (NYC == 128) return TG == 2 ? launch_wgrad<128, 2, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream) : launch_wgrad<128, 1, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+  if (TG == 4) return launch_wgrad<64, 4, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+  if (TG == 3) return launch_wgrad<64, 3, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
+  return launch_wgrad<64, 1, false, 0>(xmap, ymap, p, x_blocks, sm_count, stream);
 }
