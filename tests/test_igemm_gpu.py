@@ -10,6 +10,28 @@ from pillarnext_b200 import ops
 pytestmark = pytest.mark.gpu
 
 
+def _grid_cases(cases, skip=()):
+    """Each case as it was (same id, the device's SM count as grid budget) and again with a budget of one SM (id + "-1sm"):
+    one CTA per column block then walks every tile, carrying its smem ring and epilogue handoff from tile to tile.  Cases
+    with fewer than 3 tiles (`skip`) gain nothing from it."""
+    out = []
+    for c in cases:
+        cid = "-".join(str(v) for v in c)
+        out.append(pytest.param(*c, None, id=cid))
+        if c not in skip:
+            out.append(pytest.param(*c, 1, id=cid + "-1sm"))
+    return out
+
+
+def _use_sms(monkeypatch, sms, tiles, n_blocks):
+    """Grid budget `sms` (None: the device's) for the launches that follow; with one SM, assert that a CTA gets >= 3 tiles."""
+    if sms is None:
+        return
+    monkeypatch.setattr(ops, "sm_count", lambda: sms)
+    gx = max(1, min(sms // n_blocks, tiles))
+    assert -(-tiles // gx) >= 3, "tiles per CTA: %d tiles on %d CTAs" % (tiles, gx)
+
+
 def _close(out, ref, bf16_out):
     scale = ref.abs().max().item() + 1e-6
     tol = (2e-3 + (8e-3 if bf16_out else 0)) * scale
@@ -17,9 +39,11 @@ def _close(out, ref, bf16_out):
     assert err <= tol, "max abs err %g > tol %g (scale %g)" % (err, tol, scale)
 
 
-@pytest.mark.parametrize("M,K,N,bn", [(128, 64, 64, 64), (1000, 128, 256, 256), (333, 256, 128, 128), (5000, 64, 384, 192),
-                                      (257, 64, 16, 16), (4096, 256, 32, 32), (20000, 256, 256, 256)])
-def test_plain_gemm(M, K, N, bn):
+@pytest.mark.parametrize("M,K,N,bn,sms", _grid_cases([(128, 64, 64, 64), (1000, 128, 256, 256), (333, 256, 128, 128),
+                                                      (5000, 64, 384, 192), (257, 64, 16, 16), (4096, 256, 32, 32),
+                                                      (20000, 256, 256, 256)], skip=[(128, 64, 64, 64)]))
+def test_plain_gemm(M, K, N, bn, sms, monkeypatch):
+    _use_sms(monkeypatch, sms, -(-M // 128), N // bn)
     torch.manual_seed(M + K + N)
     A = torch.randn(M, K, device="cuda").bfloat16()
     W = (torch.randn(1, N, K, device="cuda") * 0.1).bfloat16()
@@ -38,8 +62,9 @@ def test_plain_gemm(M, K, N, bn):
     assert torch.allclose(stats[N:], (s * s).sum(0), rtol=1e-6, atol=1e-3)
 
 
-@pytest.mark.parametrize("M,Min,C,N", [(3000, 2500, 64, 64), (1500, 4000, 128, 256), (700, 700, 256, 256)])
-def test_table_gather(M, Min, C, N):
+@pytest.mark.parametrize("M,Min,C,N,sms", _grid_cases([(3000, 2500, 64, 64), (1500, 4000, 128, 256), (700, 700, 256, 256)]))
+def test_table_gather(M, Min, C, N, sms, monkeypatch):
+    _use_sms(monkeypatch, sms, -(-M // 128), N // ops.pick_block_n(N))
     torch.manual_seed(M)
     A = torch.randn(Min, C, device="cuda").bfloat16()
     W = (torch.randn(9, N, C, device="cuda") * 0.05).bfloat16()
@@ -54,9 +79,12 @@ def test_table_gather(M, Min, C, N):
     _close(out, ref, True)
 
 
-@pytest.mark.parametrize("B,H,W_,Cin,Cout,k,stride,dil", [(2, 24, 24, 64, 64, 3, 1, 1), (1, 40, 36, 256, 256, 3, 1, 6), (1, 21, 33, 128, 256, 3, 2, 1),
-                                                         (2, 16, 16, 256, 256, 1, 1, 1), (1, 48, 48, 64, 384, 3, 1, 1), (1, 50, 50, 256, 64, 3, 1, 18)])
-def test_dense_conv(B, H, W_, Cin, Cout, k, stride, dil):
+@pytest.mark.parametrize("B,H,W_,Cin,Cout,k,stride,dil,sms", _grid_cases(
+    [(2, 24, 24, 64, 64, 3, 1, 1), (1, 40, 36, 256, 256, 3, 1, 6), (1, 21, 33, 128, 256, 3, 2, 1), (2, 16, 16, 256, 256, 1, 1, 1),
+     (1, 48, 48, 64, 384, 3, 1, 1), (1, 50, 50, 256, 64, 3, 1, 18)], skip=[(1, 21, 33, 128, 256, 3, 2, 1)]))
+def test_dense_conv(B, H, W_, Cin, Cout, k, stride, dil, sms, monkeypatch):
+    Ho_, Wo_ = (H + 2 * dil * (k // 2) - dil * (k - 1) - 1) // stride + 1, (W_ + 2 * dil * (k // 2) - dil * (k - 1) - 1) // stride + 1
+    _use_sms(monkeypatch, sms, -(-B * Ho_ * Wo_ // 128), Cout // ops.pick_block_n(Cout))
     torch.manual_seed(H * W_ + Cin)
     x = torch.randn(B, Cin, H, W_, device="cuda").bfloat16()
     w = (torch.randn(Cout, Cin, k, k, device="cuda") * 0.05).bfloat16()
@@ -71,8 +99,18 @@ def test_dense_conv(B, H, W_, Cin, Cout, k, stride, dil):
 
 
 def test_conv_transpose_shuffle():
+    _conv_transpose_shuffle()
+
+
+def test_conv_transpose_shuffle_1sm(monkeypatch):
+    _conv_transpose_shuffle(monkeypatch)
+
+
+def _conv_transpose_shuffle(monkeypatch=None):
     torch.manual_seed(5)
     B, H, W_, C = 2, 12, 20, 64
+    if monkeypatch is not None:
+        _use_sms(monkeypatch, 1, -(-B * H * W_ // 128), 4 * C // ops.pick_block_n(4 * C))
     x = torch.randn(B, C, H, W_, device="cuda").bfloat16()
     w = (torch.randn(C, C, 2, 2, device="cuda") * 0.1).bfloat16()           # [Cin, Cout, kh, kw]
     ref = F.conv_transpose2d(x.float(), w.float(), stride=2)

@@ -40,11 +40,26 @@ def test_descriptor_base_offset_convention():
     assert good == ops.WIN_BASE_OFF, "flip ops.WIN_BASE_OFF to %d" % good
 
 
-@pytest.mark.parametrize("B,H,W,Cin,Cout,bn", [(2, 9, 336, 64, 384, 192), (1, 5, 130, 384, 64, 64), (2, 7, 128, 128, 128, 128),
-                                               (1, 12, 40, 256, 64, 64), (1, 3, 257, 64, 192, 192),
-                                               # Cin = 64 with block_n <= 128: weights-stationary variant
-                                               (2, 9, 336, 64, 384, 128), (1, 3, 257, 64, 128, 64)])
-def test_conv3x3_win(B, H, W, Cin, Cout, bn):
+def _grid_cases(cases):
+    """Each case as it was (same id, the device's SM count as grid budget) and again with a budget of one SM (id + "-1sm"):
+    one CTA per column block then walks every tile, carrying its smem ring and epilogue handoff from tile to tile."""
+    out = []
+    for c in cases:
+        cid = "-".join(str(v) for v in c)
+        out.append(pytest.param(*c, None, id=cid))
+        out.append(pytest.param(*c, 1, id=cid + "-1sm"))
+    return out
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,bn,sms", _grid_cases([(2, 9, 336, 64, 384, 192), (1, 5, 130, 384, 64, 64), (2, 7, 128, 128, 128, 128),
+                                                              (1, 12, 40, 256, 64, 64), (1, 3, 257, 64, 192, 192),
+                                                              # Cin = 64 with block_n <= 128: weights-stationary variant
+                                                              (2, 9, 336, 64, 384, 128), (1, 3, 257, 64, 128, 64)]))
+def test_conv3x3_win(B, H, W, Cin, Cout, bn, sms, monkeypatch):
+    if sms is not None:
+        monkeypatch.setattr(ops, "sm_count", lambda: sms)
+        tiles, gx = B * H * -(-W // 128), max(1, min(sms // (Cout // bn), B * H * -(-W // 128)))
+        assert -(-tiles // gx) >= 3, "tiles per CTA: %d tiles on %d CTAs" % (tiles, gx)
     err, stats_ok = run(B, H, W, Cin, Cout, bn, None)
     assert err < 1.2e-2, err
     assert stats_ok

@@ -22,6 +22,27 @@ def _slot_buffer(M, N):
     return buf, buf[:M, GUARD:GUARD + N]
 
 
+def _grid_cases(cases):
+    """Each case as it was (same id, the device's SM count as grid budget) and again with a budget of one SM (id + "-1sm"):
+    one CTA per column block then walks every tile, so the store warpgroup's staged / sfree handoff, its pass parity and the
+    per-CTA statistics carry over from tile to tile."""
+    out = []
+    for c in (cases if isinstance(cases[0], tuple) else [(c,) for c in cases]):
+        cid = "-".join(str(v) for v in c)
+        out.append(pytest.param(*c, None, id=cid))
+        out.append(pytest.param(*c, 1, id=cid + "-1sm"))
+    return out
+
+
+def _use_sms(monkeypatch, sms, tiles, n_blocks):
+    """Grid budget `sms` (None: the device's) for the launches that follow; with one SM, assert that a CTA gets >= 3 tiles."""
+    if sms is None:
+        return
+    monkeypatch.setattr(ops, "sm_count", lambda: sms)
+    gx = max(1, min(sms // n_blocks, tiles))
+    assert -(-tiles // gx) >= 3, "tiles per CTA: %d tiles on %d CTAs" % (tiles, gx)
+
+
 def _check_sentinel(buf, M, N):
     assert (buf[:, :GUARD] == SENTINEL).all(), "left guard columns overwritten"
     assert (buf[:, GUARD + N:] == SENTINEL).all(), "right guard columns overwritten"
@@ -71,9 +92,11 @@ def _check_bnr(bnr, plain, gated):
 # ------------------------------------------------------------------------------------------------- igemm
 # igemm stages its epilogue for BN <= 192; the BN = 256 sets run the in-register epilogue (a regression check of that path,
 # not coverage of the store warps).
-@pytest.mark.parametrize("B,H,W_,Cin,Cout,bn", [(1, 9, 37, 64, 64, 64), (2, 7, 29, 128, 128, 128), (1, 11, 31, 64, 384, 192),
-                                                (1, 13, 23, 256, 256, 256), (1, 5, 53, 64, 32, 32)])
-def test_igemm_slot_tail_stats(B, H, W_, Cin, Cout, bn):
+@pytest.mark.parametrize("B,H,W_,Cin,Cout,bn,sms", _grid_cases([(1, 9, 37, 64, 64, 64), (2, 7, 29, 128, 128, 128),
+                                                                (1, 11, 31, 64, 384, 192), (1, 13, 23, 256, 256, 256),
+                                                                (1, 5, 53, 64, 32, 32)]))
+def test_igemm_slot_tail_stats(B, H, W_, Cin, Cout, bn, sms, monkeypatch):
+    _use_sms(monkeypatch, sms, -(-B * H * W_ // 128), Cout // bn)
     torch.manual_seed(Cout + W_)
     x = torch.randn(B, Cin, H, W_, device="cuda").bfloat16()
     w = (torch.randn(Cout, Cin, 3, 3, device="cuda") * 0.05).bfloat16()
@@ -91,10 +114,11 @@ def test_igemm_slot_tail_stats(B, H, W_, Cin, Cout, bn):
     _stats_match(stats, out)
 
 
-@pytest.mark.parametrize("bn", [16, 64, 128, 256])   # store warps for 16 / 64 / 128; 256: in-register epilogue
-def test_igemm_shuffle_stats(bn):
+@pytest.mark.parametrize("bn,sms", _grid_cases([16, 64, 128, 256]))   # store warps for 16 / 64 / 128; 256: in-register epilogue
+def test_igemm_shuffle_stats(bn, sms, monkeypatch):
     torch.manual_seed(11)
     B, H, W_, C = 2, 9, 23, 64          # 414 input pixels: the last tile is partial
+    _use_sms(monkeypatch, sms, -(-B * H * W_ // 128), 4 * C // bn)
     x = torch.randn(B, C, H, W_, device="cuda").bfloat16()
     w = (torch.randn(C, C, 2, 2, device="cuda") * 0.1).bfloat16()
     ref = F.conv_transpose2d(x.float(), w.float(), stride=2).permute(0, 2, 3, 1).reshape(-1, C)
@@ -110,10 +134,11 @@ def test_igemm_shuffle_stats(bn):
     _stats_match(stats, out)
 
 
-@pytest.mark.parametrize("Cout,bn", [(64, 64), (128, 128), (192, 192), (256, 256)])   # 256: in-register epilogue
-def test_igemm_bnr_gate(Cout, bn):
+@pytest.mark.parametrize("Cout,bn,sms", _grid_cases([(64, 64), (128, 128), (192, 192), (256, 256)]))   # 256: in-register epilogue
+def test_igemm_bnr_gate(Cout, bn, sms, monkeypatch):
     torch.manual_seed(Cout)
     M, Min, Cin = 1000, 900, 128
+    _use_sms(monkeypatch, sms, -(-M // 128), Cout // bn)
     A = torch.randn(Min, Cin, device="cuda").bfloat16()
     W = (torch.randn(9, Cout, Cin, device="cuda") * 0.05).bfloat16()
     nbr = torch.randint(-Min // 3, Min, (M, 9), device="cuda", dtype=torch.int32).clamp(min=-1)
@@ -127,9 +152,11 @@ def test_igemm_bnr_gate(Cout, bn):
 
 
 # ------------------------------------------------------------------------------------------------- igemm_win
-@pytest.mark.parametrize("B,H,W_,Cin,Cout,bn", [(1, 5, 200, 64, 64, 64), (2, 3, 150, 64, 128, 128), (1, 4, 140, 128, 128, 128),
-                                                (1, 3, 130, 128, 192, 192), (1, 6, 90, 256, 64, 64)])
-def test_win_slot_tail_stats(B, H, W_, Cin, Cout, bn):
+@pytest.mark.parametrize("B,H,W_,Cin,Cout,bn,sms", _grid_cases([(1, 5, 200, 64, 64, 64), (2, 3, 150, 64, 128, 128),
+                                                                (1, 4, 140, 128, 128, 128), (1, 3, 130, 128, 192, 192),
+                                                                (1, 6, 90, 256, 64, 64)]))
+def test_win_slot_tail_stats(B, H, W_, Cin, Cout, bn, sms, monkeypatch):
+    _use_sms(monkeypatch, sms, B * H * -(-W_ // 128), Cout // bn)
     torch.manual_seed(Cout + W_ + Cin)
     x = torch.randn(B, Cin, H, W_, device="cuda").bfloat16()
     w = (torch.randn(Cout, Cin, 3, 3, device="cuda") * 0.05).bfloat16()
@@ -146,10 +173,11 @@ def test_win_slot_tail_stats(B, H, W_, Cin, Cout, bn):
     _stats_match(stats, out)
 
 
-@pytest.mark.parametrize("Cin,Cout,bn", [(64, 128, 128), (128, 64, 64)])
-def test_win_bnr_gate(Cin, Cout, bn):
+@pytest.mark.parametrize("Cin,Cout,bn,sms", _grid_cases([(64, 128, 128), (128, 64, 64)]))
+def test_win_bnr_gate(Cin, Cout, bn, sms, monkeypatch):
     torch.manual_seed(Cin + Cout)
     B, H, W_ = 1, 5, 170
+    _use_sms(monkeypatch, sms, B * H * -(-W_ // 128), Cout // bn)
     M = B * H * W_
     x = torch.randn(M, Cin, device="cuda").bfloat16()
     wp = (torch.randn(9, Cout, Cin, device="cuda") * 0.05).bfloat16()

@@ -16,12 +16,36 @@ def _close(out, ref, extra=0.0):
     assert err <= (3e-3 + extra) * scale, "max abs err %g (scale %g)" % (err, scale)
 
 
-@pytest.mark.parametrize("M,Min,Cx,Cy", [(5000, 4000, 64, 64), (20000, 20000, 256, 256), (3000, 3000, 128, 64), (7777, 9000, 384, 64),
-                                         (700, 900, 256, 128), (100, 100, 256, 1536), (6000, 5000, 64, 384), (4100, 4100, 128, 192)])
-def test_wgrad_table(M, Min, Cx, Cy):
+def _split_cases(cases):
+    """Each case as it was (same id, the device's SM count sizes the K splits) and again with a budget of one SM (id +
+    "-1sm": one split, or two, of many rows each) and of 4096 SMs (id + "-4096sm": the most splits the rows allow)."""
+    out = []
+    for c in cases:
+        cid = "-".join(str(v) for v in c)
+        out += [pytest.param(*c, None, id=cid), pytest.param(*c, 1, id=cid + "-1sm"), pytest.param(*c, 4096, id=cid + "-4096sm")]
+    return out
+
+
+def _use_sms(monkeypatch, sms, cx, cy, taps, M):
+    """Grid budget `sms` (None: the device's) for the wgrad launches that follow, and the split count it must give."""
+    if sms is None:
+        return
+    monkeypatch.setattr(ops, "sm_count", lambda: sms)
+    splits = ops.lib().pnx_wgrad_splits(cx, cy, taps, M, ops.sm_count())
+    if sms == 1:
+        assert splits <= 2, "%d K splits with one SM" % splits
+    else:
+        assert splits * 1024 >= M, "%d K splits of %d rows: not the most the rows allow" % (splits, M)
+
+
+@pytest.mark.parametrize("M,Min,Cx,Cy,sms", _split_cases([(5000, 4000, 64, 64), (20000, 20000, 256, 256), (3000, 3000, 128, 64),
+                                                           (7777, 9000, 384, 64), (700, 900, 256, 128), (100, 100, 256, 1536),
+                                                           (6000, 5000, 64, 384), (4100, 4100, 128, 192)]))
+def test_wgrad_table(M, Min, Cx, Cy, sms, monkeypatch):
     """X = dOut (direct, M rows), Y = In (gathered through a random neighbour table with holes)."""
     torch.manual_seed(M + Cx)
     T = 9
+    _use_sms(monkeypatch, sms, Cx, Cy, T, M)
     nbr = torch.randint(-Min // 3, Min, (M, T), device="cuda", dtype=torch.int32).clamp(min=-1)
     X = torch.randn(M, Cx, device="cuda").bfloat16()
     Y = torch.randn(Min, Cy, device="cuda").bfloat16()
@@ -40,8 +64,11 @@ def test_wgrad_table(M, Min, Cx, Cy):
     _close(d1[0], X.float().t() @ Y1.float())
 
 
-@pytest.mark.parametrize("B,H,W_,Cin,Cout,k,stride,dil", [(2, 24, 24, 64, 64, 3, 1, 1), (1, 40, 36, 256, 256, 3, 1, 6), (1, 21, 33, 128, 256, 3, 2, 1), (2, 16, 16, 256, 256, 1, 1, 1)])
-def test_wgrad_dense_conv(B, H, W_, Cin, Cout, k, stride, dil):
+@pytest.mark.parametrize("B,H,W_,Cin,Cout,k,stride,dil,sms", _split_cases([(2, 24, 24, 64, 64, 3, 1, 1), (1, 40, 36, 256, 256, 3, 1, 6),
+                                                                        (1, 21, 33, 128, 256, 3, 2, 1), (2, 16, 16, 256, 256, 1, 1, 1)]))
+def test_wgrad_dense_conv(B, H, W_, Cin, Cout, k, stride, dil, sms, monkeypatch):
+    Ho_, Wo_ = (H + 2 * dil * (k // 2) - dil * (k - 1) - 1) // stride + 1, (W_ + 2 * dil * (k // 2) - dil * (k - 1) - 1) // stride + 1
+    _use_sms(monkeypatch, sms, Cout, Cin, k * k, B * Ho_ * Wo_)
     torch.manual_seed(H + Cin)
     x = torch.randn(B, Cin, H, W_, device="cuda").bfloat16()
     w = torch.zeros(Cout, Cin, k, k, device="cuda", requires_grad=True)
@@ -57,6 +84,12 @@ def test_wgrad_dense_conv(B, H, W_, Cin, Cout, k, stride, dil):
     ops.wgrad(dy_rows, Cout, x_rows, Cin, M, k * k, dW, dense=(Ho, Wo, H, W_, k, stride, dil, pad) if k > 1 else None)
     got = dW.view(k, k, Cout, Cin).permute(2, 3, 0, 1)
     _close(got, w.grad)
+
+
+@pytest.mark.parametrize("sms", [1, 4096])
+def test_wgrad_conv_transpose_grid(sms, monkeypatch):
+    _use_sms(monkeypatch, sms, 64, 64, 4, 2 * 12 * 20)
+    test_wgrad_conv_transpose()
 
 
 def test_wgrad_conv_transpose():

@@ -36,7 +36,17 @@ def _run(X, Y, B, H, W, cx=None, cy=None):
     return dW
 
 
-@pytest.mark.parametrize("B,H,W,cx,cy", [
+def _split_cases(cases):
+    """Each case as it was (same id, the device's SM count sizes the K splits) and again with a budget of one SM (id +
+    "-1sm": one split, or two, of many rows each) and of 4096 SMs (id + "-4096sm": the most splits the rows allow)."""
+    out = []
+    for c in cases:
+        cid = "-".join(str(v) for v in c)
+        out += [pytest.param(*c, None, id=cid), pytest.param(*c, 1, id=cid + "-1sm"), pytest.param(*c, 4096, id=cid + "-4096sm")]
+    return out
+
+
+@pytest.mark.parametrize("B,H,W,cx,cy,sms", _split_cases([
     (1, 24, 336, 384, 64),     # the head's 64 -> 384 convolution at its 336-pixel width (chunk 112, no padding)
     (2, 20, 176, 128, 64),     # 176: not a multiple of the chunk (96)
     (1, 9, 101, 128, 128),     # odd width: not a multiple of 16, the gather path runs
@@ -44,8 +54,12 @@ def _run(X, Y, B, H, W, cx=None, cy=None):
     (2, 12, 80, 128, 256),
     (2, 12, 80, 64, 64),       # 64-channel X: each consumer warpgroup takes two shifts of the window
     (1, 10, 144, 64, 192),
-])
-def test_window_wgrad_matches_fp64(B, H, W, cx, cy):
+]))
+def test_window_wgrad_matches_fp64(B, H, W, cx, cy, sms, monkeypatch):
+    if sms is not None:
+        monkeypatch.setattr(ops, "sm_count", lambda: sms)
+        splits, M = ops.lib().pnx_wgrad_splits(cx, cy, 9, B * H * W, sms), B * H * W
+        assert (splits <= 2) if sms == 1 else (splits * 1024 >= M), "%d K splits of %d rows with %d SMs" % (splits, M, sms)
     torch.manual_seed(B * 1000 + H + W + cx + cy)
     X = torch.randn(B * H * W, cx, device="cuda").bfloat16()
     Y = torch.randn(B * H * W, cy, device="cuda").bfloat16()
