@@ -406,6 +406,37 @@ int pnx_global_aug(const float* points, int n, const float* boxes, int B, int M,
 int pnx_global_aug_host(const float* points, int n, const float* boxes, int B, int M, const double* aug,
                         float* points_out, float* boxes_out);
 
+/* ---------------------------------------------------------------- ground-truth database sampling
+ * pnx_gt_sample: the reference's DataBaseSamplerV2 acceptance (sample_class_v2) and paste (datasets/base.py:77-96) for a
+ * collated batch, given the candidates the data-loader workers drew.
+ *   points [n, 6] (batch_idx, x, y, z, intensity, time); scene boxes [B, M, 9], classes [B, M] (-1 = padding),
+ *   box_trig [B, M, 2] = numpy's fp32 (cos, sin) of each yaw;
+ *   cand_boxes [B, S, 9], cand_classes [B, S] (-1 = padding; a class call is a run of equal ids), cand_trig [B, S, 4] =
+ *   (numpy cos, numpy sin, libm cosf, sinf) of each yaw; cand_points [P, 5] (x, y, z relative to the box centre,
+ *   intensity, time), candidate (b, s) owning rows cand_off[b S + s] .. cand_off[b S + s + 1] - 1 (cand_off [B S + 1]).
+ * Outputs (new memory):
+ *   points_out [n + P, 6]: per frame in frame order, the accepted objects' points (xyz + box centre) in acceptance order,
+ *     then the frame's scene points outside every accepted box, in their input order; rows [*count, n + P) get batch
+ *     index B and zeros.  A scene point whose batch index is not an integer in [0, B) is dropped.
+ *   boxes_out [B, M + S, 9], classes_out [B, M + S]: the real scene boxes, the accepted ones, then padding (class -1,
+ *     size 1); accepted [B, S] (may be NULL): 1 where the candidate was accepted; count [1]: valid rows of points_out.
+ * Arithmetic and quirks: csrc/gt_sample.cu.  Four launches on `stream`, no host sync, no allocation: `workspace` holds
+ * pnx_gt_sample_workspace(n, B, S) bytes of device memory (no initialisation needed).  B <= 512.  The host twin takes
+ * HOST memory and needs no workspace.  pnx_points_in_boxes_host is the point test alone (box_np_ops.points_in_rbbox):
+ * inside [n, m] bytes for points with x, y, z at the start of `stride`-float rows, 9-column boxes, and trig [m, 2] =
+ * (cosf, sinf) of each yaw. */
+long long pnx_gt_sample_workspace(int n, int B, int S);
+int pnx_gt_sample(const float* points, int n, const float* boxes, const int* classes, const float* box_trig, int B, int M,
+                  const float* cand_boxes, const int* cand_classes, const float* cand_trig, int S, const float* cand_points,
+                  const int* cand_off, int P, float* points_out, float* boxes_out, int* classes_out, int* accepted,
+                  int* count, void* workspace, cudaStream_t stream);
+int pnx_gt_sample_host(const float* points, int n, const float* boxes, const int* classes, const float* box_trig, int B,
+                       int M, const float* cand_boxes, const int* cand_classes, const float* cand_trig, int S,
+                       const float* cand_points, const int* cand_off, int P, float* points_out, float* boxes_out,
+                       int* classes_out, int* accepted, int* count);
+int pnx_points_in_boxes_host(const float* points, int n, int stride, const float* boxes, const float* trig, int m,
+                             unsigned char* inside);
+
 #ifdef __cplusplus
 }
 #endif

@@ -91,9 +91,14 @@ _SIGS = {
     # global training augmentation (rotation, scaling, translation, flip) of points and raw boxes
     "pnx_global_aug": [P, I, P, I, I, P, P, P, P],
     "pnx_global_aug_host": [P, I, P, I, I, P, P, P],
+    # ground-truth database sampling: collision test, scene-point removal and paste
+    "pnx_gt_sample_workspace": [I, I, I],
+    "pnx_gt_sample": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P, P, P],
+    "pnx_gt_sample_host": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P],
+    "pnx_points_in_boxes_host": [P, I, I, P, P, I, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
-            "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong,
+            "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,
             "pnx_det_iou_bev_host": ctypes.c_float, "pnx_aligned_iou3d_host": ctypes.c_float}
 
 

@@ -724,7 +724,27 @@ class SingleStageDetector(nn.Module):
         out["points"], out["gt_boxes_raw"] = points, boxes
         return out
 
+    GTS_KEYS = ("gts_boxes", "gts_classes", "gts_trig", "gts_points", "gts_offsets", "gt_trig")
+
+    def gt_sample(self, example):
+        """Ground-truth database sampling on the GPU: the candidates the loader drew (gts_* keys of scenes.collate,
+        det3d.datasets.pipelines.sample_ops) go through the reference's collision test, and the accepted ones are
+        pasted by ops.gt_sample -- points, raw boxes and classes -- what the reference's data-loader workers do in numpy
+        before the global augmentation.  Returns the example without the gts_* keys."""
+        if "hm" in example:
+            raise ValueError("the example already carries assigned labels (hm); ground-truth sampling (gts_*) must be "
+                             "applied to the raw boxes before label assignment")
+        e = example
+        points, boxes, classes, _, _ = ops.gt_sample(e["points"], e["gt_boxes_raw"], e["gt_classes"], e["gt_trig"],
+                                                     e["gts_boxes"], e["gts_classes"], e["gts_trig"], e["gts_points"],
+                                                     e["gts_offsets"])
+        out = {k: v for k, v in example.items() if k not in self.GTS_KEYS}
+        out["points"], out["gt_boxes_raw"], out["gt_classes"] = points, boxes, classes
+        return out
+
     def training_step(self, example):
+        if "gts_boxes" in example:
+            example = self.gt_sample(example)
         if "aug" in example:
             example = self.global_aug(example)
         if "hm" not in example and "gt_boxes_raw" in example:

@@ -840,6 +840,45 @@ def global_aug(points, gt_boxes, aug):
     return pts_out, box_out
 
 
+def gt_sample(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, cand_trig, cand_points, cand_offsets):
+    """Ground-truth database sampling on the GPU (pnx_gt_sample, include/pnx.h): the reference's collision test,
+    scene-point removal and paste for the candidates scenes.collate packed (gts_* keys; all CUDA tensors):
+    points [N, 6] fp32, scene boxes [B, M, 9] fp32, classes [B, M] int32, gt_trig [B, M, 2] fp32, candidates
+    [B, S, 9] / [B, S] / [B, S, 4], cand_points [P, 5] fp32, cand_offsets [B S + 1] int32 ->
+    (points [N + P, 6], boxes [B, M + S, 9], classes [B, M + S] int32, accepted [B, S] int32, count [1] int32 cuda).
+    The rows past `count` have batch index B, which the voxelizers drop; the host does not wait for the count.  Frames
+    stay in order, each with its pasted objects' points first, so frame-sorted input stays frame-sorted."""
+    def want(t, dtype, shape, what):
+        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
+            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
+    assert points.dim() == 2 and gt_boxes.dim() == 3 and cand_boxes.dim() == 3, "points [N, 6], boxes [B, M, 9], [B, S, 9]"
+    (n, _), (B, M, _), S = points.shape, gt_boxes.shape, cand_boxes.shape[1]
+    P = cand_points.shape[0]
+    want(points, torch.float32, (n, 6), "points")
+    want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes")
+    want(gt_classes, torch.int32, (B, M), "gt_classes")
+    want(gt_trig, torch.float32, (B, M, 2), "gt_trig")
+    want(cand_boxes, torch.float32, (B, S, 9), "cand_boxes")
+    want(cand_classes, torch.int32, (B, S), "cand_classes")
+    want(cand_trig, torch.float32, (B, S, 4), "cand_trig")
+    want(cand_points, torch.float32, (P, 5), "cand_points")
+    want(cand_offsets, torch.int32, (B * S + 1,), "cand_offsets")
+    args = [t.contiguous() for t in (points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, cand_trig,
+                                     cand_points, cand_offsets)]
+    dev = points.device
+    pts_out = torch.empty((n + P, 6), dtype=torch.float32, device=dev)
+    box_out = torch.empty((B, M + S, 9), dtype=torch.float32, device=dev)
+    cls_out = torch.empty((B, M + S), dtype=torch.int32, device=dev)
+    accepted = torch.empty((B, S), dtype=torch.int32, device=dev)
+    count = torch.empty(1, dtype=torch.int32, device=dev)
+    ws = torch.empty(max(4, lib().pnx_gt_sample_workspace(n, B, S)), dtype=torch.uint8, device=dev)
+    p, b, c, t, cb, cc, ct, cp, co = args
+    _count(1)
+    check(lib().pnx_gt_sample(ptr(p), n, ptr(b), ptr(c), ptr(t), B, M, ptr(cb), ptr(cc), ptr(ct), S, ptr(cp), ptr(co), P,
+                              ptr(pts_out), ptr(box_out), ptr(cls_out), ptr(accepted), ptr(count), ptr(ws), stream()))
+    return pts_out, box_out, cls_out, accepted, count
+
+
 def aligned_iou3d(boxes_a, boxes_b):
     """[n, 7] x [n, 7] fp32 (x, y, z, dx, dy, dz, heading) -> [n] aligned 3-D IoU (iou3d_nms_utils.py:45-87)."""
     assert boxes_a.shape == boxes_b.shape and boxes_a.shape[-1] == 7 and boxes_a.is_cuda

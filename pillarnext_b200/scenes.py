@@ -10,7 +10,9 @@ SyntheticSceneDataset follows det3d/datasets/base.py (`__len__`, `__getitem__`, 
 base.py:48-108) as far as the hot path needs it; label assignment is NOT done on the CPU workers (assign.py) -- the
 collated batch carries the raw boxes and the detector builds the targets on the GPU (pnx_assign_labels, row F3).
 Global augmentation (`augmentation=`, base.py:97-99) is split the same way: the drop-in transforms of
-det3d.datasets.pipelines.augmentation draw their parameters here and the detector applies them on the GPU."""
+det3d.datasets.pipelines.augmentation draw their parameters here and the detector applies them on the GPU.  So is
+ground-truth database sampling (`sampler=`, base.py:36-39, 72-96): det3d.datasets.pipelines.sample_ops draws the
+candidate objects here, and the detector runs the collision test, the point removal and the paste on the GPU."""
 import numpy as np
 import torch
 
@@ -100,16 +102,27 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     splits are disjoint seed ranges.
 
     augmentation: dict of `_target_` nodes (or transform objects) applied to every frame in dict order after the scene
-    is made, as the reference's BaseDataset does; each appends its record to the frame's `aug` list."""
+    is made, as the reference's BaseDataset does; each appends its record to the frame's `aug` list.
+
+    sampler: the reference's `_partial_` DataBaseSamplerV2 node (or a callable returning a sampler), called once here
+    as base.py does.  Each frame then gets a `gts` record before augmentation draws anything: the candidate objects
+    (sample_ops.DataBaseSamplerV2.sample_all; none drawn = zero candidates) and numpy's (cos, sin) of the scene boxes'
+    yaws.  root_path is where the sampler node's `${data.train_dataset.root_path}` points (the gt database)."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
-                 augmentation=None, **_):
+                 augmentation=None, sampler=None, root_path=None, **_):
         self.cfg, self.n_frames, self.seed0, self.n_points, self.n_boxes = cfg, int(n_frames), int(seed0), int(n_points), int(n_boxes)
         self.test_mode = test_mode
         self.class_names = [n for t in cfg["tasks"] for n in t]
         if augmentation and test_mode:
             raise ValueError("augmentation is a training transform: a test_mode dataset must not set it")
         self.augmentations = hydra_lite.instantiate(augmentation) if augmentation else None
+        if sampler and test_mode:
+            raise ValueError("sampler is a training transform: a test_mode dataset must not set it")
+        self.root_path = root_path
+        self.sampler = None
+        if sampler:
+            self.sampler = (hydra_lite.instantiate(sampler) if isinstance(sampler, dict) else sampler)()
 
     def __len__(self):
         return self.n_frames
@@ -118,10 +131,28 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
         cls = np.array([self.class_names.index(n) for n in names], dtype=np.int32)
         res = {"points": pts, "gt_boxes_raw": boxes, "gt_classes": cls, "token": "scene_%d" % (self.seed0 + i)}
+        if self.sampler is not None:
+            res["gts"] = self._candidates(boxes, names)
         if self.augmentations is not None:
             for aug in self.augmentations.values():
                 res = aug(res)
         return res
+
+    def _candidates(self, boxes, names):
+        from det3d.datasets.pipelines.sample_ops import numpy_trig
+        rec = self.sampler.sample_all(boxes, np.array(names))
+        if rec is None:
+            rec = {"gt_names": np.zeros(0, dtype=str), "gt_boxes": np.zeros((0, 9), np.float32),
+                   "points": np.zeros((0, 5), np.float32), "num_points": np.zeros(0, np.int64),
+                   "trig": np.zeros((0, 4), np.float32)}
+        if rec["points"].shape[1] != 5:
+            raise ValueError("the sampler's point_dim must be 5 (x, y, z, intensity, time), got %d" % rec["points"].shape[1])
+        unknown = sorted(set(rec["gt_names"]) - set(self.class_names))
+        if unknown:
+            raise ValueError("sampled classes %s are not classes of this dataset" % unknown)
+        return {"boxes": rec["gt_boxes"], "classes": np.array([self.class_names.index(n) for n in rec["gt_names"]], np.int32),
+                "points": rec["points"], "num_points": rec["num_points"], "trig": rec["trig"],
+                "scene_trig": numpy_trig(boxes)}
 
     def ground_truth(self):
         gts = {}
@@ -139,7 +170,12 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
 def collate(batch_list):
     """loader/collate.py:6-35 for this dataset: points get the frame index prepended; raw boxes are padded to the
     longest frame (class -1 = padding).  Frames with augmentation records add aug [B, 4, 4] float64: frame i's records
-    (code, p0, p1, p2) in slots 0.., the rest zero (empty)."""
+    (code, p0, p1, p2) in slots 0.., the rest zero (empty).  Frames with sampling records (`gts`) add, with S the most
+    candidates of any frame (at least 1):
+      gts_boxes [B, S, 9] fp32, gts_classes [B, S] int32 (-1 = padding), gts_trig [B, S, 4] fp32   the candidates
+      gts_points [P, 5] fp32, gts_offsets [B S + 1] int32    their stored points; candidate (b, s) owns rows
+                                                             gts_offsets[b S + s] .. gts_offsets[b S + s + 1] - 1
+      gt_trig [B, M, 2] fp32                                 numpy's (cos, sin) of the scene boxes' yaws"""
     pts = [np.pad(b["points"], ((0, 0), (1, 0)), mode="constant", constant_values=i) for i, b in enumerate(batch_list)]
     m = max(1, max(len(b["gt_classes"]) for b in batch_list))
     boxes = np.zeros((len(batch_list), m, 9), dtype=np.float32)
@@ -160,4 +196,29 @@ def collate(batch_list):
             if rec:
                 aug[i, :len(rec)] = rec
         out["aug"] = torch.tensor(aug)
+    if any("gts" in b for b in batch_list):
+        if not all("gts" in b for b in batch_list):
+            raise ValueError("either every frame of a batch carries a sampling record (gts) or none does")
+        B = len(batch_list)
+        s = max(1, max(len(b["gts"]["classes"]) for b in batch_list))
+        cb = np.zeros((B, s, 9), dtype=np.float32)
+        cb[:, :, 3:6] = 1.0
+        cc = np.full((B, s), -1, dtype=np.int32)
+        ct = np.zeros((B, s, 4), dtype=np.float32)
+        ct[:, :, 0], ct[:, :, 2] = 1.0, 1.0
+        st = np.zeros((B, m, 2), dtype=np.float32)
+        st[:, :, 0] = 1.0
+        counts = np.zeros((B, s), dtype=np.int64)
+        for i, b in enumerate(batch_list):
+            g = b["gts"]
+            k = len(g["classes"])
+            cb[i, :k], cc[i, :k], ct[i, :k], counts[i, :k] = g["boxes"], g["classes"], g["trig"], g["num_points"]
+            st[i, :len(g["scene_trig"])] = g["scene_trig"]
+        off = np.concatenate([[0], np.cumsum(counts.reshape(-1))])
+        if off[-1] + len(out["points"]) >= 2 ** 31 - 1:
+            raise ValueError("too many points in one batch for int32 offsets")
+        pts = [b["gts"]["points"] for b in batch_list]
+        out.update(gts_boxes=torch.tensor(cb), gts_classes=torch.tensor(cc), gts_trig=torch.tensor(ct),
+                   gts_points=torch.tensor(np.concatenate(pts, 0).astype(np.float32).reshape(-1, 5)),
+                   gts_offsets=torch.tensor(off.astype(np.int32)), gt_trig=torch.tensor(st))
     return out
