@@ -437,6 +437,35 @@ int pnx_gt_sample_host(const float* points, int n, const float* boxes, const int
 int pnx_points_in_boxes_host(const float* points, int n, int stride, const float* boxes, const float* trig, int m,
                              unsigned char* inside);
 
+/* ---------------------------------------------------------------- Waymo-style evaluation (pillarnext_b200/evaluate_waymo.py)
+ * pnx_eval_count_points: counts [B, M] int32 = number of points inside each ground-truth box, with the reference's
+ * points_in_boxes_jit test (the one pnx_gt_sample uses).  points [n, stride >= 4] with (batch_idx, x, y, z) in columns
+ * 0-3 (a row whose batch index is not an integer in [0, B) is skipped); boxes [B, M, 9] (x, y, z, dx, dy, dz, vx, vy,
+ * yaw), classes [B, M] (-1 = padding, count 0), trig [B, M, 2] = libm (cosf, sinf) of each yaw.  Exact integer counts.
+ * pnx_eval_match: the greedy score-ordered match of detections to ground truth, per (frame, class) segment s = f C + c.
+ *   det_boxes [n_det, 9], det_trig [n_det, 2] = (cos, sin) of each yaw; order [n_det] int64 = detection indices sorted
+ *   by segment, then by descending score, ties by lower index; segment s holds order[seg_start[s] ..
+ *   seg_start[s] + seg_count[s]) (seg_start / seg_count [B C] int32); gt_boxes [B, M, 9], gt_classes [B, M] in [0, C)
+ *   or -1 (padding), gt_trig [B, M, 2] = (cos, sin) of each yaw; thresholds [C] fp32 IoU thresholds; M <= 4096.
+ *   Each detection in order takes the unmatched box of its segment with the highest aligned 3-D IoU (boxes_iou3d_gpu
+ *   arithmetic, detection first), ties to the lower box index, if that IoU >= thresholds[c].  Outputs per detection
+ *   (indexed like det_boxes): match = the box index j within its frame or -1, iou = the highest IoU over the boxes still
+ *   unmatched when it was visited (0 if none), heading = 1 - min(|d|, 2 pi - |d|) / pi of the yaw difference d for a
+ *   match, else 0.
+ * Both run on `stream` with no host sync and no workspace; the _host twins take HOST memory. */
+int pnx_eval_count_points(const float* points, long long n, int stride, const float* boxes, const int* classes,
+                          const float* trig, int B, int M, int* counts, cudaStream_t stream);
+int pnx_eval_count_points_host(const float* points, long long n, int stride, const float* boxes, const int* classes,
+                               const float* trig, int B, int M, int* counts);
+int pnx_eval_match(const float* det_boxes, const float* det_trig, long long n_det, const long long* order,
+                   const int* seg_start, const int* seg_count, const float* gt_boxes, const int* gt_classes,
+                   const float* gt_trig, int B, int M, int C, const float* thresholds, int* match, float* iou,
+                   float* heading, cudaStream_t stream);
+int pnx_eval_match_host(const float* det_boxes, const float* det_trig, long long n_det, const long long* order,
+                        const int* seg_start, const int* seg_count, const float* gt_boxes, const int* gt_classes,
+                        const float* gt_trig, int B, int M, int C, const float* thresholds, int* match, float* iou,
+                        float* heading);
+
 #ifdef __cplusplus
 }
 #endif

@@ -96,6 +96,11 @@ _SIGS = {
     "pnx_gt_sample": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P, P, P],
     "pnx_gt_sample_host": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P],
     "pnx_points_in_boxes_host": [P, I, I, P, P, I, P],
+    # Waymo-style evaluation: point counts per ground-truth box and the greedy score-ordered match
+    "pnx_eval_count_points": [P, L, I, P, P, P, I, I, P, P],
+    "pnx_eval_count_points_host": [P, L, I, P, P, P, I, I, P],
+    "pnx_eval_match": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P, P],
+    "pnx_eval_match_host": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,

@@ -30,6 +30,7 @@
 
 #include <vector>
 
+#include "box_geom.cuh"
 #include "pnx_common.cuh"
 
 namespace {
@@ -40,30 +41,6 @@ constexpr int kGeo = 12;        // BEV geometry: x0 y0 .. x3 y3, standup min x, 
 constexpr int kPtThreads = 512;  // mark / write block size (both kernels must partition the points alike)
 constexpr int kPtWarps = kPtThreads / 32;
 constexpr int kSelThreads = 256;
-
-__host__ __device__ inline float mul_f(float a, float b) {
-#ifdef __CUDA_ARCH__
-  return __fmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-__host__ __device__ inline float add_f(float a, float b) {
-#ifdef __CUDA_ARCH__
-  return __fadd_rn(a, b);
-#else
-  return a + b;
-#endif
-}
-__host__ __device__ inline float sub_f(float a, float b) {
-#ifdef __CUDA_ARCH__
-  return __fsub_rn(a, b);
-#else
-  return a - b;
-#endif
-}
-__host__ __device__ inline float min_f(float a, float b) { return b < a ? b : a; }
-__host__ __device__ inline float max_f(float a, float b) { return b > a ? b : a; }
 
 // center_to_corner_box2d of box (x, y, dx, dy from a 9-column box) with numpy's (c, s), + corner_to_standup_nd
 __host__ __device__ inline void bev_geometry(const float* box, float c, float s, float* g) {
@@ -112,20 +89,6 @@ __host__ __device__ inline bool collide(const float* b, const float* q) {
     }
   }
   return corners_inside(b, q) || corners_inside(q, b);
-}
-
-// points_in_boxes_jit for one (point, box) pair; box is 9-column (yaw last), (c, s) = libm cosf / sinf of the yaw
-__host__ __device__ inline bool point_in_box(float x, float y, float z, const float* box, float c, float s) {
-  if (!((double)fabsf(sub_f(z, box[2])) <= (double)box[5] / 2.0)) return false;
-  const float sx = sub_f(x, box[0]), sy = sub_f(y, box[1]);
-  const float lx = add_f(mul_f(sx, c), mul_f(sy, s));
-  const float ly = add_f(mul_f(-sx, s), mul_f(sy, c));
-  return (double)fabsf(lx) <= (double)box[3] / 2.0 && (double)fabsf(ly) <= (double)box[4] / 2.0;
-}
-
-// frame index of a point row: an integer in [0, B), else -1 (the row is dropped)
-__host__ __device__ inline int frame_of(float f, int B) {
-  return (f >= 0.0f && f < (float)B && f == floorf(f)) ? (int)f : -1;
 }
 
 struct Args {

@@ -15,7 +15,7 @@
 // Double-flip testing (pnx_det_*_flip4): the same three passes over the 4B-frame head output of a flip4_points batch
 // (flip.cu); the decode reads the four copies of each pixel at their mirrored positions and merges them
 // (det_decode_pixel_flip4), so no flipped or averaged copy of any head map is ever written.
-// Provenance note: the rotated-rectangle overlap routines below (cross3, rect_cross, in_box2d, seg_intersection,
+// Provenance note: the rotated-rectangle overlap routines (box_geom.cuh: cross3, rect_cross, in_box2d, seg_intersection,
 // det_box_overlap, det_iou_bev) deliberately follow the ARITHMETIC of the reference's own device code,
 // det3d/core/iou3d_nms/src/iou3d_nms_kernel.cu:39-235 (and its host twin iou3d_cpu.cpp), statement by statement -- same
 // operation order, same 1e-2 margin, same angular ordering of the polygon vertices: the keep / suppress decision of every
@@ -25,6 +25,7 @@
 // Hot loop character: HBM-bound single pass (1) and a few hundred thousand polygon clips (2) -- no tensor-core work.
 #include <math.h>
 
+#include "box_geom.cuh"
 #include "pnx_common.cuh"
 
 namespace {
@@ -162,112 +163,6 @@ __host__ __device__ inline bool det_decode_pixel_flip4(const DetParams& p, long 
 // boxes always agree.
 __host__ __device__ inline bool det_decode(const DetParams& p, long long m, float* box, float* score, int* label) {
   return p.flip4 ? det_decode_pixel_flip4(p, m, box, score, label) : det_decode_pixel(p, m, box, score, label);
-}
-
-// ------------------------------------------------------------------ rotated BEV IoU (iou3d_cpu.cpp:62-237 algorithm:
-// edge crossings + contained corners, sorted by angle about their centroid, shoelace area)
-struct P2 { float x, y; };
-
-__host__ __device__ inline float cross3(const P2& p1, const P2& p2, const P2& p0) {
-  return (p1.x - p0.x) * (p2.y - p0.y) - (p2.x - p0.x) * (p1.y - p0.y);
-}
-
-__host__ __device__ inline bool rect_cross(const P2& p1, const P2& p2, const P2& q1, const P2& q2) {
-  return fminf(p1.x, p2.x) <= fmaxf(q1.x, q2.x) && fminf(q1.x, q2.x) <= fmaxf(p1.x, p2.x) &&
-         fminf(p1.y, p2.y) <= fmaxf(q1.y, q2.y) && fminf(q1.y, q2.y) <= fmaxf(p1.y, p2.y);
-}
-
-// box7 = (x, y, z, dx, dy, dz, heading)
-__host__ __device__ inline bool in_box2d(const float* box, const P2& p) {
-  const float kMargin = 1e-2f;
-  const float c = cosf(-box[6]), s = sinf(-box[6]);
-  const float rx = (p.x - box[0]) * c + (p.y - box[1]) * (-s);
-  const float ry = (p.x - box[0]) * s + (p.y - box[1]) * c;
-  return fabsf(rx) < box[3] / 2 + kMargin && fabsf(ry) < box[4] / 2 + kMargin;
-}
-
-__host__ __device__ inline bool seg_intersection(const P2& p1, const P2& p0, const P2& q1, const P2& q0, P2* ans) {
-  const float kEps = 1e-8f;
-  if (!rect_cross(p0, p1, q0, q1)) return false;
-  const float s1 = cross3(q0, p1, p0), s2 = cross3(p1, q1, p0), s3 = cross3(p0, q1, q0), s4 = cross3(q1, p1, q0);
-  if (!(s1 * s2 > 0 && s3 * s4 > 0)) return false;
-  const float s5 = cross3(q1, p1, p0);
-  if (fabsf(s5 - s1) > kEps) {
-    ans->x = (s5 * q0.x - s1 * q1.x) / (s5 - s1);
-    ans->y = (s5 * q0.y - s1 * q1.y) / (s5 - s1);
-  } else {
-    const float a0 = p0.y - p1.y, b0 = p1.x - p0.x, c0 = p0.x * p1.y - p1.x * p0.y;
-    const float a1 = q0.y - q1.y, b1 = q1.x - q0.x, c1 = q0.x * q1.y - q1.x * q0.y;
-    const float D = a0 * b1 - a1 * b0;
-    ans->x = (b0 * c1 - b1 * c0) / D;
-    ans->y = (a1 * c0 - a0 * c1) / D;
-  }
-  return true;
-}
-
-__host__ __device__ inline void box_corners(const float* box, P2* c5) {
-  const float hx = box[3] / 2, hy = box[4] / 2;
-  const float ca = cosf(box[6]), sa = sinf(box[6]);
-  const float px[4] = {-hx, hx, hx, -hx}, py[4] = {-hy, -hy, hy, hy};
-  for (int k = 0; k < 4; ++k) {
-    c5[k].x = px[k] * ca + py[k] * (-sa) + box[0];
-    c5[k].y = px[k] * sa + py[k] * ca + box[1];
-  }
-  c5[4] = c5[0];
-}
-
-__host__ __device__ inline float det_box_overlap(const float* a, const float* b) {
-  P2 ca[5], cb[5], pts[16];
-  box_corners(a, ca);
-  box_corners(b, cb);
-  int cnt = 0;
-  float sx = 0.f, sy = 0.f;
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
-      P2 q;
-      if (cnt < 16 && seg_intersection(ca[i + 1], ca[i], cb[j + 1], cb[j], &q)) {
-        sx += q.x; sy += q.y;
-        pts[cnt++] = q;
-      }
-    }
-  for (int k = 0; k < 4; ++k) {
-    if (cnt < 16 && in_box2d(a, cb[k])) { sx += cb[k].x; sy += cb[k].y; pts[cnt++] = cb[k]; }
-    if (cnt < 16 && in_box2d(b, ca[k])) { sx += ca[k].x; sy += ca[k].y; pts[cnt++] = ca[k]; }
-  }
-  if (cnt == 0) return 0.f;
-  const float cx = sx / cnt, cy = sy / cnt;
-  float ang[16];
-  for (int k = 0; k < cnt; ++k) ang[k] = atan2f(pts[k].y - cy, pts[k].x - cx);
-  for (int j = 0; j < cnt - 1; ++j)
-    for (int i = 0; i < cnt - j - 1; ++i)
-      if (ang[i] > ang[i + 1]) {
-        const P2 t = pts[i]; pts[i] = pts[i + 1]; pts[i + 1] = t;
-        const float ta = ang[i]; ang[i] = ang[i + 1]; ang[i + 1] = ta;
-      }
-  float area = 0.f;
-  for (int k = 0; k < cnt - 1; ++k) {
-    const float ax = pts[k].x - pts[0].x, ay = pts[k].y - pts[0].y;
-    const float bx = pts[k + 1].x - pts[0].x, by = pts[k + 1].y - pts[0].y;
-    area += ax * by - ay * bx;
-  }
-  return fabsf(area) / 2.0f;
-}
-
-__host__ __device__ inline float det_iou_bev(const float* a, const float* b) {
-  const float sa = a[3] * a[4], sb = b[3] * b[4];
-  const float so = det_box_overlap(a, b);
-  return so / fmaxf(sa + sb - so, 1e-8f);
-}
-
-// aligned 3-D IoU of two (x, y, z, dx, dy, dz, heading) boxes: BEV overlap x height overlap over the union volume
-// (reference det3d/core/iou3d_nms/iou3d_nms_utils.py:45-87 boxes_aligned_iou3d_gpu; training target of the `iou` head)
-__host__ __device__ inline float det_aligned_iou3d(const float* a, const float* b) {
-  const float a_max = a[2] + a[5] / 2, a_min = a[2] - a[5] / 2;
-  const float b_max = b[2] + b[5] / 2, b_min = b[2] - b[5] / 2;
-  const float oh = fmaxf(fminf(a_max, b_max) - fmaxf(a_min, b_min), 0.f);
-  const float o3 = det_box_overlap(a, b) * oh;
-  const float va = a[3] * a[4] * a[5], vb = b[3] * b[4] * b[5];
-  return o3 / fmaxf(va + vb - o3, 1e-6f);
 }
 
 // (x, y, z, dx, dy, dz, vx, vy, yaw) -> (x, y, z, dx, dy, dz, yaw): boxes_for_nms = box[:, [0,1,2,3,4,5,-1]]

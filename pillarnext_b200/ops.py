@@ -887,3 +887,60 @@ def aligned_iou3d(boxes_a, boxes_b):
     _count(1)
     check(lib().pnx_aligned_iou3d(ptr(a), ptr(b), a.shape[0], ptr(out), stream()))
     return out
+
+
+# --------------------------------------------------------------------------------- Waymo-style evaluation
+def eval_count_points(points, boxes, classes, trig):
+    """Points inside each ground-truth box (pnx_eval_count_points, include/pnx.h), with the reference's
+    points_in_boxes_jit test: points [N, >= 4] fp32 (batch_idx, x, y, z, ...), boxes [B, M, 9] fp32, classes [B, M]
+    int32 (-1 = padding), trig [B, M, 2] fp32 libm (cosf, sinf) of each yaw, all CUDA -> counts [B, M] int32 cuda."""
+    def want(t, dtype, shape, what):
+        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
+            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
+    assert points.dim() == 2 and points.shape[1] >= 4 and boxes.dim() == 3, "points [N, >= 4], boxes [B, M, 9]"
+    B, M = boxes.shape[:2]
+    want(points, torch.float32, points.shape, "points")
+    want(boxes, torch.float32, (B, M, 9), "boxes")
+    want(classes, torch.int32, (B, M), "classes")
+    want(trig, torch.float32, (B, M, 2), "trig")
+    points = points if points.stride(1) == 1 else points.contiguous()
+    row = points.stride(0) if points.shape[0] > 1 else points.shape[1]    # an empty or one-row tensor's stride is arbitrary
+    boxes, classes, trig = boxes.contiguous(), classes.contiguous(), trig.contiguous()
+    counts = torch.empty((B, M), dtype=torch.int32, device=boxes.device)
+    _count(1)
+    check(lib().pnx_eval_count_points(ptr(points), points.shape[0], row, ptr(boxes), ptr(classes), ptr(trig), B, M,
+                                      ptr(counts), stream()))
+    return counts
+
+
+def eval_match(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, thresholds):
+    """Greedy score-ordered matching per (frame, class) segment (pnx_eval_match, include/pnx.h), all CUDA:
+    det_boxes [D, 9] fp32, det_trig [D, 2] fp32 (cos, sin) of each yaw, order [D] int64 (detections sorted by segment
+    f C + c, then descending score, ties by lower index), seg_start / seg_count [B C] int32, gt_boxes [B, M, 9] fp32,
+    gt_classes [B, M] int32 (-1 = padding), gt_trig [B, M, 2] fp32, thresholds [C] fp32 ->
+    (match [D] int32 box index within the frame or -1, iou [D] fp32, heading accuracy [D] fp32)."""
+    def want(t, dtype, shape, what):
+        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
+            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
+    assert det_boxes.dim() == 2 and gt_boxes.dim() == 3 and thresholds.dim() == 1, "det_boxes [D, 9], gt_boxes [B, M, 9]"
+    D, (B, M), C = det_boxes.shape[0], gt_boxes.shape[:2], thresholds.shape[0]
+    want(det_boxes, torch.float32, (D, 9), "det_boxes")
+    want(det_trig, torch.float32, (D, 2), "det_trig")
+    want(order, torch.int64, (D,), "order")
+    want(seg_start, torch.int32, (B * C,), "seg_start")
+    want(seg_count, torch.int32, (B * C,), "seg_count")
+    want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes")
+    want(gt_classes, torch.int32, (B, M), "gt_classes")
+    want(gt_trig, torch.float32, (B, M, 2), "gt_trig")
+    want(thresholds, torch.float32, (C,), "thresholds")
+    args = [t.contiguous() for t in (det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig,
+                                     thresholds)]
+    db, dt, od, ss, sc, gb, gc, gt, th = args
+    dev = det_boxes.device
+    match = torch.empty(D, dtype=torch.int32, device=dev)
+    iou = torch.empty(D, dtype=torch.float32, device=dev)
+    heading = torch.empty(D, dtype=torch.float32, device=dev)
+    _count(1)
+    check(lib().pnx_eval_match(ptr(db), ptr(dt), D, ptr(od), ptr(ss), ptr(sc), ptr(gb), ptr(gc), ptr(gt), B, M, C, ptr(th),
+                               ptr(match), ptr(iou), ptr(heading), stream()))
+    return match, iou, heading

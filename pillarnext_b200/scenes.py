@@ -107,12 +107,18 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     sampler: the reference's `_partial_` DataBaseSamplerV2 node (or a callable returning a sampler), called once here
     as base.py does.  Each frame then gets a `gts` record before augmentation draws anything: the candidate objects
     (sample_ops.DataBaseSamplerV2.sample_all; none drawn = zero candidates) and numpy's (cos, sin) of the scene boxes'
-    yaws.  root_path is where the sampler node's `${data.train_dataset.root_path}` points (the gt database)."""
+    yaws.  root_path is where the sampler node's `${data.train_dataset.root_path}` points (the gt database).
+
+    metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map) or "waymo" (evaluate_waymo.waymo_metrics,
+    AP / APH at LEVEL_1 and LEVEL_2; ground_truth() then also hands over each frame's points)."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
-                 augmentation=None, sampler=None, root_path=None, **_):
+                 augmentation=None, sampler=None, root_path=None, metric="nuscenes", **_):
         self.cfg, self.n_frames, self.seed0, self.n_points, self.n_boxes = cfg, int(n_frames), int(seed0), int(n_points), int(n_boxes)
         self.test_mode = test_mode
+        if metric not in ("nuscenes", "waymo"):
+            raise ValueError("metric must be 'nuscenes' or 'waymo', got %r" % (metric,))
+        self.metric = metric
         self.class_names = [n for t in cfg["tasks"] for n in t]
         if augmentation and test_mode:
             raise ValueError("augmentation is a training transform: a test_mode dataset must not set it")
@@ -157,12 +163,17 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     def ground_truth(self):
         gts = {}
         for i in range(self.n_frames):
-            _, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
+            pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
             gts["scene_%d" % (self.seed0 + i)] = {"boxes": boxes, "names": names}
+            if self.metric == "waymo":
+                gts["scene_%d" % (self.seed0 + i)]["points"] = pts
         return gts
 
     def evaluation(self, detections, output_dir=None, testset=False):
         """The hook the reference trainer calls at the end of val_epoch (base.py:48-51, trainer.py:165-184)."""
+        if self.metric == "waymo":
+            from .evaluate_waymo import waymo_metrics
+            return waymo_metrics(self.ground_truth(), detections, self.class_names)
         from .evaluate import detection_map
         return detection_map(self.ground_truth(), detections, self.class_names)
 
