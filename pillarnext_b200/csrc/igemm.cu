@@ -11,10 +11,12 @@
 // CTA persistent over 128-row tiles: warpgroup 0 writes the gathered row of every (tap, row) of a tile into shared
 // memory, then per K stage loads the weight tile by TMA and gathers the 128 A rows with 16-byte cp.async (index -1 = zero
 // fill) into the 128B-swizzled layout; warpgroups 1-2 each run wgmma on 64 rows into registers.  Staged variants
-// (Cfg::kStaged) have a fourth warpgroup: the consumers round the tile into shared memory and go back to their MMAs, and
-// warpgroup 3 stores it and sums its statistics meanwhile (gemm_epilogue.cuh).  The others -- BN = 256, whose 128
-// accumulator registers per thread do not fit the 128 a 512-thread CTA allows, and the fp32 variant F = 2 -- keep the
-// whole epilogue on warpgroups 1-2.
+// (Cfg::kStaged) have a fourth warpgroup: the consumers write the tile into shared memory and go back to their MMAs, and
+// warpgroup 3 stores it and sums its statistics meanwhile (gemm_epilogue.cuh).  At BN = 256 (Cfg::kWide) the consumers'
+// 128 accumulator registers per thread do not fit the 128 a 512-thread CTA allows: setmaxnreg moves registers from the
+// producer and store warpgroups to them, and the store threads keep the statistic slots in registers, which frees the
+// shared memory for the whole-tile staging buffer and 3 stages.  Only fp32 output at BN = 192 and 256 (the split mode)
+// keeps the whole epilogue on warpgroups 1-2.
 #include "gemm_epilogue.cuh"
 
 namespace {
@@ -43,24 +45,28 @@ struct IgemmParams {
 
 constexpr uint32_t kABytes = 128 * 128;  // one A stage: 128 rows x 64 bf16
 constexpr int kProducerRegs = 56, kConsumerRegs = 224;  // unstaged variants (384 threads): 128 * 56 + 256 * 224 <= 65536
+constexpr int kWideStoreRegs = 88, kWideConsumerRegs = 184;  // kWide (512 threads): 128 * (56 + 88) + 256 * 184 = 65536
 
 template <int BN, int F>
 struct Cfg {
-  static constexpr bool kStaged = F != 2 && BN <= 192;
+  static constexpr bool kStaged = F != 2 || BN <= 128;  // fp32 at BN = 192 would spill at 128 registers per thread
+  static constexpr bool kWide = kStaged && BN == 256;  // setmaxnreg split, statistic slots in the store threads' registers
   static constexpr int kThreads = kStaged ? 512 : 384;  // + the store warpgroup
   static constexpr uint32_t kBBytes = BN * 128;
   static constexpr int kTbl = 128 * 9;  // ints of the per-tile index table [tap][row]
-  static constexpr int kFixed = 1024 + kTbl * 4 + 256 + (2 * pnx::kEpiWarps + 5) * BN * 4;
+  static constexpr int kStatFloats = kWide ? 0 : 2 * pnx::kEpiWarps * BN;  // s_stat
+  static constexpr int kFixed = 1024 + kTbl * 4 + 256 + (kStatFloats + 5 * BN) * 4;
   static constexpr int kStageBytes = (int)(kABytes + kBBytes);
   static constexpr int kAvail = 227 * 1024 - kFixed;
   // staged epilogue: the whole tile at once, or in two column halves where that would leave fewer than 3 stages
-  static constexpr int kPasses = !kStaged ? 1 : ((kAvail - pnx::Staging<BN, 1>::kBytes) / kStageBytes >= 3 ? 1 : 2);
-  static constexpr int kStgBytes = !kStaged ? 0 : pnx::Staging<BN, kPasses>::kBytes;
+  static constexpr int kPasses = !kStaged ? 1 : ((kAvail - pnx::StagingF<BN, 1, F>::kBytes) / kStageBytes >= 3 ? 1 : 2);
+  static constexpr int kStgBytes = !kStaged ? 0 : pnx::StagingF<BN, kPasses, F>::kBytes;
   static constexpr int kStagesRaw = (kAvail - kStgBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
   static constexpr size_t kSmem = (size_t)kFixed + (size_t)kStgBytes + (size_t)kStages * kStageBytes;
   static_assert(kStages >= 3, "pipeline depth");
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
+  static_assert(!kWide || kPasses == 1, "register statistic slots need the whole tile staged");
 };
 
 __device__ __forceinline__ void named_bar_sync(int id, int n) {
@@ -86,7 +92,7 @@ __global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __
   uint64_t* staged = empty + kStages;  // the consumers' 256 threads wrote a staging pass
   uint64_t* sfree = staged + 1;        // the store warpgroup has drained it
   float* s_stat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 256);  // [8 warps][2][BN] per-channel sums
-  float* s_bias = s_stat + pnx::kEpiWarps * 2 * BN;                                  // [BN] bias of this CTA's columns
+  float* s_bias = s_stat + C::kStatFloats;                                           // [BN] bias of this CTA's columns
   float* s_bnc = s_bias + BN;                                                        // [4][BN] fused BN-backward affine
 
   const int wg = threadIdx.x >> 7;
@@ -105,7 +111,7 @@ __global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __
   }
   if (p.bias)
     for (int c = threadIdx.x; c < BN; c += blockDim.x) s_bias[c] = p.bias[n0 + c];
-  for (int c = threadIdx.x; c < pnx::kEpiWarps * 2 * BN; c += blockDim.x) s_stat[c] = 0.f;
+  for (int c = threadIdx.x; c < C::kStatFloats; c += blockDim.x) s_stat[c] = 0.f;
   if (F == 1)
     for (int c = threadIdx.x; c < BN; c += blockDim.x) {
       const int gc = n0 + c;
@@ -120,19 +126,27 @@ __global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __
   if (wg == 3) {
     // ---------------------------------------------------------------- store warpgroup (staged variants): drains the tiles
     if constexpr (C::kStaged) {
+      if constexpr (C::kWide) pnx::regs_dealloc<kWideStoreRegs>();
       const int stid = threadIdx.x - 384;
       uint32_t spass = 0;
+      float4 r_stat[pnx::kEpiWarps];  // kWide: the statistic slots of column pair stid
+#pragma unroll
+      for (int w = 0; w < pnx::kEpiWarps; ++w) r_stat[w] = make_float4(0.f, 0.f, 0.f, 0.f);
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const long long row0 = (long long)tile * 128;
-        pnx::gemm_epilogue_drain<BN, F, kPasses>(p.epi, row0, (int)min((long long)128, (long long)p.M - row0), n0, stg, s_stat,
-                                                 s_bnc, staged, sfree, spass, stid, 128, 2);
+        pnx::gemm_epilogue_drain<BN, F, kPasses, C::kWide>(p.epi, row0, (int)min((long long)128, (long long)p.M - row0), n0, stg,
+                                                           s_stat, s_bnc, staged, sfree, spass, stid, 128, 2, r_stat);
       }
-      named_bar_sync(2, 128);
-      pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, stid, 128);
+      if constexpr (C::kWide) {
+        pnx::gemm_epilogue_flush_regs<BN, F>(p.epi, n0, r_stat, p.bnr_red, p.bnr_C, stid);
+      } else {
+        named_bar_sync(2, 128);
+        pnx::gemm_epilogue_flush<BN, F>(p.epi, n0, s_stat, p.bnr_red, p.bnr_C, stid, 128);
+      }
     }
   } else if (wg == 0) {
     // ---------------------------------------------------------------- producer
-    if constexpr (!C::kStaged) pnx::regs_dealloc<kProducerRegs>();
+    if constexpr (!C::kStaged || C::kWide) pnx::regs_dealloc<kProducerRegs>();
     const int ptid = threadIdx.x;
     const int sub = ptid & 7, rsub = ptid >> 3;  // a warp instruction copies 4 whole 128-byte rows
     const int hw = p.Hout * p.Wout;
@@ -191,6 +205,7 @@ __global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __
   } else {
     // ---------------------------------------------------------------- consumers: wgmma + epilogue
     if constexpr (!C::kStaged) pnx::regs_alloc<kConsumerRegs>();
+    if constexpr (C::kWide) pnx::regs_alloc<kWideConsumerRegs>();
     uint32_t spass = 0;
     const int half = wg - 1;  // rows [64 * half, 64 * half + 64) of every tile
     int stage = 0;
@@ -208,9 +223,20 @@ __global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __
         const uint32_t a_base = pnx::smem_u32(sA + (size_t)stage * kABytes) + half * 64 * 128;
         const uint32_t b_base = pnx::smem_u32(sB + (size_t)stage * kBBytes);
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          pnx::Wgmma<BN, 0, 0>::mma(acc, pnx::make_smem_desc_sw128(a_base + k * 32, 16, 1024),
-                                    pnx::make_smem_desc_sw128(b_base + k * 32, 16, 1024), (kc > 0 || k > 0) ? 1u : 0u);
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = pnx::make_smem_desc_sw128(a_base + k * 32, 16, 1024);
+          const uint32_t accumulate = (kc > 0 || k > 0) ? 1u : 0u;
+          if constexpr (C::kWide) {
+            // ptxas sizes one instruction's operands by the launch bound (128 registers at 512 threads), and an
+            // m64n256 wgmma needs 154: two m64n128 on the column halves, same per-element sums
+#pragma unroll
+            for (int nh = 0; nh < 2; ++nh)
+              pnx::Wgmma<128, 0, 0>::mma(*reinterpret_cast<float(*)[64]>(acc + 64 * nh), da,
+                                         pnx::make_smem_desc_sw128(b_base + nh * 128 * 128 + k * 32, 16, 1024), accumulate);
+          } else {
+            pnx::Wgmma<BN, 0, 0>::mma(acc, da, pnx::make_smem_desc_sw128(b_base + k * 32, 16, 1024), accumulate);
+          }
+        }
         pnx::wgmma_commit();
         pnx::wgmma_wait<1>();  // the previous stage's MMAs are done: release it
         if (kc > 0 && lane == 0) pnx::mbar_arrive(&empty[prev]);
@@ -223,7 +249,7 @@ __global__ void __launch_bounds__(Cfg<BN, F>::kThreads, 1) igemm_kernel(const __
       const long long row0 = (long long)tile * 128;
       const int nvalid = (int)min((long long)128, (long long)p.M - row0);
       if constexpr (C::kStaged)
-        pnx::gemm_epilogue_stage<BN, kPasses>(acc, p.epi, row0, nvalid, half, n0, s_bias, stg, staged, sfree, spass);
+        pnx::gemm_epilogue_stage<BN, kPasses, F>(acc, p.epi, row0, nvalid, half, n0, s_bias, stg, staged, sfree, spass);
       else
         pnx::gemm_epilogue<BN, F>(acc, p.epi, row0, nvalid, half, n0, s_bias, s_stat, s_bnc);
     }
