@@ -466,6 +466,24 @@ int pnx_eval_match_host(const float* det_boxes, const float* det_trig, long long
                         const float* gt_trig, int B, int M, int C, const float* thresholds, int* match, float* iou,
                         float* heading);
 
+/* ------------------------------------------------ nuScenes detection score (pillarnext_b200/evaluate_nuscenes.py)
+ * pnx_eval_match_center: the centre-distance match of the nuScenes detection benchmark, per (frame, class) segment
+ *   s = f C + c and per distance threshold.  det_boxes [n_det, 9] (x, y first); order [n_det] int64 = detection indices
+ *   sorted by segment, then in visit order (descending score, ties to the later detection); segment s holds
+ *   order[seg_start[s] .. seg_start[s] + seg_count[s]) (seg_start / seg_count [B C] int32); gt_boxes [B, M, 9],
+ *   gt_classes [B, M] in [0, C) or -1 (padding or filtered out); dist_ths [T] fp64 metres, 1 <= T <= 8; M <= 4096.
+ *   For each threshold independently, each detection in order takes the not yet matched box of its segment with the
+ *   smallest centre distance sqrt(dx^2 + dy^2) (fp64 differences of the fp32 coordinates), ties to the lower box index,
+ *   if that distance is < dist_ths[t].  Output match [T, n_det] int32 (column indexed like det_boxes): the box index j
+ *   within the frame, or -1.
+ * Runs on `stream` with no host sync and no workspace; the _host twin takes HOST memory. */
+int pnx_eval_match_center(const float* det_boxes, long long n_det, const long long* order, const int* seg_start,
+                          const int* seg_count, const float* gt_boxes, const int* gt_classes, int B, int M, int C,
+                          const double* dist_ths, int T, int* match, cudaStream_t stream);
+int pnx_eval_match_center_host(const float* det_boxes, long long n_det, const long long* order, const int* seg_start,
+                               const int* seg_count, const float* gt_boxes, const int* gt_classes, int B, int M, int C,
+                               const double* dist_ths, int T, int* match);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,6 +101,9 @@ _SIGS = {
     "pnx_eval_count_points_host": [P, L, I, P, P, P, I, I, P],
     "pnx_eval_match": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P, P],
     "pnx_eval_match_host": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P],
+    # nuScenes detection score: the centre-distance match, per threshold
+    "pnx_eval_match_center": [P, L, P, P, P, P, P, I, I, I, P, I, P, P],
+    "pnx_eval_match_center_host": [P, L, P, P, P, P, P, I, I, I, P, I, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,

@@ -944,3 +944,31 @@ def eval_match(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_cl
     check(lib().pnx_eval_match(ptr(db), ptr(dt), D, ptr(od), ptr(ss), ptr(sc), ptr(gb), ptr(gc), ptr(gt), B, M, C, ptr(th),
                                ptr(match), ptr(iou), ptr(heading), stream()))
     return match, iou, heading
+
+
+# --------------------------------------------------------------------------------- nuScenes detection score
+def eval_match_center(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, dist_ths):
+    """Centre-distance matching per (frame, class) segment and distance threshold (pnx_eval_match_center,
+    include/pnx.h), all CUDA: det_boxes [D, 9] fp32, order [D] int64 (detections sorted by segment f C + c, then in
+    visit order), seg_start / seg_count [B C] int32, gt_boxes [B, M, 9] fp32, gt_classes [B, M] int32 in [0, C) (-1 =
+    padding or filtered out), C = n_classes, dist_ths [T] fp64 -> match [T, D] int32, the box index within the frame
+    or -1."""
+    def want(t, dtype, shape, what):
+        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
+            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
+    assert det_boxes.dim() == 2 and gt_boxes.dim() == 3 and dist_ths.dim() == 1, "det_boxes [D, 9], gt_boxes [B, M, 9]"
+    D, (B, M), T, C = det_boxes.shape[0], gt_boxes.shape[:2], dist_ths.shape[0], int(n_classes)
+    want(det_boxes, torch.float32, (D, 9), "det_boxes")
+    want(order, torch.int64, (D,), "order")
+    want(seg_start, torch.int32, (B * C,), "seg_start")
+    want(seg_count, torch.int32, (B * C,), "seg_count")
+    want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes")
+    want(gt_classes, torch.int32, (B, M), "gt_classes")
+    want(dist_ths, torch.float64, (T,), "dist_ths")
+    db, od, ss, sc, gb, gc, th = [t.contiguous() for t in (det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes,
+                                                            dist_ths)]
+    match = torch.empty((T, D), dtype=torch.int32, device=det_boxes.device)
+    _count(1)
+    check(lib().pnx_eval_match_center(ptr(db), D, ptr(od), ptr(ss), ptr(sc), ptr(gb), ptr(gc), B, M, C, ptr(th), T,
+                                      ptr(match), stream()))
+    return match

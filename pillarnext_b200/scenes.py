@@ -109,15 +109,16 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     (sample_ops.DataBaseSamplerV2.sample_all; none drawn = zero candidates) and numpy's (cos, sin) of the scene boxes'
     yaws.  root_path is where the sampler node's `${data.train_dataset.root_path}` points (the gt database).
 
-    metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map) or "waymo" (evaluate_waymo.waymo_metrics,
-    AP / APH at LEVEL_1 and LEVEL_2; ground_truth() then also hands over each frame's points)."""
+    metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map), "waymo" (evaluate_waymo.waymo_metrics,
+    AP / APH at LEVEL_1 and LEVEL_2) or "nds" (evaluate_nuscenes.nuscenes_metrics, the nuScenes detection score with
+    its true-positive errors).  For "waymo" and "nds" ground_truth() also hands over each frame's points."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
                  augmentation=None, sampler=None, root_path=None, metric="nuscenes", **_):
         self.cfg, self.n_frames, self.seed0, self.n_points, self.n_boxes = cfg, int(n_frames), int(seed0), int(n_points), int(n_boxes)
         self.test_mode = test_mode
-        if metric not in ("nuscenes", "waymo"):
-            raise ValueError("metric must be 'nuscenes' or 'waymo', got %r" % (metric,))
+        if metric not in ("nuscenes", "waymo", "nds"):
+            raise ValueError("metric must be 'nuscenes', 'waymo' or 'nds', got %r" % (metric,))
         self.metric = metric
         self.class_names = [n for t in cfg["tasks"] for n in t]
         if augmentation and test_mode:
@@ -165,7 +166,7 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         for i in range(self.n_frames):
             pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
             gts["scene_%d" % (self.seed0 + i)] = {"boxes": boxes, "names": names}
-            if self.metric == "waymo":
+            if self.metric in ("waymo", "nds"):
                 gts["scene_%d" % (self.seed0 + i)]["points"] = pts
         return gts
 
@@ -174,6 +175,9 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         if self.metric == "waymo":
             from .evaluate_waymo import waymo_metrics
             return waymo_metrics(self.ground_truth(), detections, self.class_names)
+        if self.metric == "nds":
+            from .evaluate_nuscenes import nuscenes_metrics
+            return nuscenes_metrics(self.ground_truth(), detections, self.class_names)
         from .evaluate import detection_map
         return detection_map(self.ground_truth(), detections, self.class_names)
 
