@@ -264,20 +264,10 @@ def run_device(pk, point_budget=POINT_BUDGET):
 def run_host(pk, point_budget=POINT_BUDGET):
     """The same counts and match through the host twins (pnx_eval_count_points_host, pnx_eval_match_center_host): the
     CPU tests' path to the product logic."""
-    from ._lib import check, lib
-    A = lambda a: a.ctypes.data                                                                   # noqa: E731
-
-    def count(p, b, c, t):
-        out = np.zeros(c.shape, np.int32)
-        check(lib().pnx_eval_count_points_host(A(p), len(p), 4, A(b), A(c), A(t), c.shape[0], c.shape[1], A(out)))
-        return out
-    counts = count_points(pk, count, point_budget)
-    B, M, C, D = pk["B"], pk["M"], pk["C"], len(pk["det_scores"])
-    ths = np.array(DIST_THS, np.float64)
-    match = np.zeros((len(ths), D), np.int32)
-    classes = evaluated_classes(pk, counts)
-    check(lib().pnx_eval_match_center_host(A(pk["det_boxes"]), D, A(pk["order"]), A(pk["seg_start"]), A(pk["seg_count"]),
-                                           A(pk["gt_boxes"]), A(classes), B, M, C, A(ths), len(ths), A(match)))
+    from . import ops
+    counts = count_points(pk, ops.eval_count_points_host, point_budget)
+    match = ops.eval_match_center_host(pk["det_boxes"], pk["order"], pk["seg_start"], pk["seg_count"], pk["gt_boxes"],
+                                       evaluated_classes(pk, counts), pk["C"], np.array(DIST_THS, np.float64))
     return counts, match
 
 

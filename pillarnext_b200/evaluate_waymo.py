@@ -146,18 +146,11 @@ def run_device(pk):
 
 def run_host(pk):
     """The same counts and matches through the host twins (pnx_eval_*_host): the CPU tests' path to the product logic."""
-    from ._lib import check, lib
-    A = lambda a: a.ctypes.data                                                                   # noqa: E731
-    B, M, C, D = pk["B"], pk["M"], pk["C"], len(pk["det_scores"])
-    pts = np.ascontiguousarray(pk["points"])
-    counts = np.zeros((B, M), np.int32)
-    check(lib().pnx_eval_count_points_host(A(pts), len(pts), 4, A(pk["gt_boxes"]), A(pk["gt_classes"]), A(pk["count_trig"]),
-                                           B, M, A(counts)))
+    from . import ops
+    counts = ops.eval_count_points_host(pk["points"], pk["gt_boxes"], pk["gt_classes"], pk["count_trig"])
     order = np.argsort(pk["keys"], kind="stable").astype(np.int64)
-    match, iou, heading = np.zeros(D, np.int32), np.zeros(D, np.float32), np.zeros(D, np.float32)
-    check(lib().pnx_eval_match_host(A(pk["det_boxes"]), A(pk["det_trig"]), D, A(order), A(pk["seg_start"]),
-                                    A(pk["seg_count"]), A(pk["gt_boxes"]), A(pk["gt_classes"]), A(pk["gt_trig"]), B, M, C,
-                                    A(pk["thresholds"]), A(match), A(iou), A(heading)))
+    match, iou, heading = ops.eval_match_host(pk["det_boxes"], pk["det_trig"], order, pk["seg_start"], pk["seg_count"],
+                                              pk["gt_boxes"], pk["gt_classes"], pk["gt_trig"], pk["thresholds"])
     return counts, match, iou, heading
 
 

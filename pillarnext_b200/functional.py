@@ -542,30 +542,21 @@ class BNActFn(torch.autograd.Function):
         dy = dy.contiguous()
         dx = torch.empty(M, C, dtype=torch.bfloat16, device=dy.device)
         dres = torch.empty(M, C, dtype=torch.bfloat16, device=dy.device) if ctx.has_res else None
-        from ._lib import check, lib, ptr, stream
         info = ctx.info
         fused = info is not None and info.fused
         # without a residual the ReLU mask is recomputed from x_raw (one row-matrix read less per pass)
         ysrc = y if ctx.has_res else None
-        yp, ys = (ptr(ysrc), ysrc.stride(0)) if ysrc is not None else (None, 8)
         if fused:
             local = info.red          # the reduce pass ran in the epilogue of the GEMM that produced dy (= gated g)
             info.red, info.fused = None, False
         else:
-            local = ops.zeros(2 * C, torch.float64, dy.device)
-            ops._count(1)
-            check(lib().pnx_bn_bwd_reduce(ptr(dy), dy.stride(0), yp, ys, ptr(x_raw), x_raw.stride(0), M, C, ptr(mean), ptr(invstd),
-                                          1 if ctx.relu else 0, ptr(scale), ptr(shift), ptr(local), stream()))
+            local = ops.bn_bwd_reduce(dy, ysrc, x_raw, M, C, mean, invstd, ctx.relu, (scale, shift))
         red = local
         if ctx.sync:                  # SyncBatchNorm: the two sums over all ranks (dgamma / dbeta stay local, DDP averages them)
             red = local.clone()
             dist.all_reduce(red)
-        ops._count(1)
-        check(lib().pnx_bn_bwd_apply(ptr(dy), dy.stride(0), yp, ys, ptr(x_raw), x_raw.stride(0), M, C, ptr(mean), ptr(invstd),
-                                     ptr(gamma), ptr(red), float(max(ctx.count, 1)), ptr(ctx.count_dev) if ctx.count_dev is not None else None,
-                                     1 if (ctx.relu and not fused) else 0,
-                                     ptr(scale), ptr(shift), ptr(dx), dx.stride(0), ptr(dres) if dres is not None else None,
-                                     dres.stride(0) if dres is not None else 8, 0, stream()))
+        ops.bn_bwd_apply(dy, ysrc, x_raw, M, C, mean, invstd, gamma, red, ctx.count, ctx.relu and not fused, (scale, shift), dx,
+                         dres=dres, count_dev=ctx.count_dev)
         r = local.float()
         return dx, None, r[C:], r[:C], dres, None, None, None, None
 
@@ -804,30 +795,17 @@ class CenterLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, meta, *outs):
-        import ctypes
-        from ._lib import check, lib, ptr, stream
         T = len(outs)
         dev = outs[0].device
         acc = ops.zeros((T, 16), torch.float64, dev)
         res = torch.empty(T, 16, dtype=torch.float32, device=dev)
         total = torch.empty(1, dtype=torch.float32, device=dev)
         douts = []
-        cw = (ctypes.c_float * 10)(*meta["code_weights"])
         for t, out in enumerate(outs):
             m = meta["tasks"][t]
-            ex = m["labels"]
-            dout = torch.empty_like(out)
-            ops._count(2)
-            check(lib().pnx_center_loss_task(ptr(out), ptr(dout), ptr(ex["hm"]), ptr(ex["anno_box"]), ptr(ex["ind"]),
-                                             ptr(ex["mask"]), ptr(ex["cat"]), ptr(ex["gt_boxes"]), m["B"], m["H"], m["W"],
-                                             m["npad"], m["C"], m["M"], m["off"]["reg"], m["off"]["height"], m["off"]["dim"],
-                                             m["off"]["rot"], m["off"]["vel"], m["off"]["hm"], m["sx"], m["sy"], m["ox"], m["oy"],
-                                             meta["weight"], ctypes.cast(cw, ctypes.c_void_p), 1 if meta["with_reg_iou"] else 0,
-                                             ptr(acc[t]), stream()))
-            douts.append(dout)
-        ops._count(1)
-        check(lib().pnx_center_loss_finalize(ptr(acc), T, ptr(meta["weights_dev"]), ptr(meta["code_w_dev"]),
-                                             ptr(meta["with_iou_dev"]), ptr(res), ptr(total), stream()))
+            douts.append(ops.center_loss_task(out, torch.empty_like(out), m["labels"], m, meta["weight"], meta["code_weights"],
+                                              meta["with_reg_iou"], acc[t]))
+        ops.center_loss_finalize(acc, meta["weights_dev"], meta["code_w_dev"], meta["with_iou_dev"], res, total)
         ctx.douts = douts
         ctx.mark_non_differentiable(res)
         return total[0], res
@@ -853,7 +831,6 @@ class HeadFinalConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, y, wb, bias, B, H, W, bn_src=None, n_used=16):
-        from ._lib import check, lib, ptr, stream
         split = _split()
         ctx.bn_src = bn_src if not split else None
         M, cin = y.shape[0], y.shape[1] // (_P() if split else 1)
@@ -866,16 +843,14 @@ class HeadFinalConvFn(torch.autograd.Function):
         Z = torch.empty(M, NZ, dtype=torch.float32, device=y.device)
         ops.igemm(y, M, wz, 1, cin, NZ, Z, block_n=NZ, segs=ops.split_segments() if split else None, a_lo_off=cin if split else 0)
         ctx.split = split
-        out = torch.empty(M, 16, dtype=torch.float32, device=y.device)
-        ops._count(1)
-        check(lib().pnx_tap_gather_sum(ptr(Z), NZ, cpt, ptr(bias.detach().float().contiguous()), B, H, W, ptr(out), stream()))
+        out = ops.tap_gather_sum(Z, cpt, bias.detach().float().contiguous(), B, H, W,
+                                 torch.empty(M, 16, dtype=torch.float32, device=y.device))
         ctx.save_for_backward(y, wz)
         ctx.geo = (B, H, W, cin, cpt, NZ)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        from ._lib import check, lib, ptr, stream
         y, wz = ctx.saved_tensors
         B, H, W, cin, cpt, NZ = ctx.geo
         M = y.shape[0]
@@ -888,9 +863,7 @@ class HeadFinalConvFn(torch.autograd.Function):
 
         if ctx.split:
             P = _P()
-            dZ = torch.empty(M, P * NZ, dtype=torch.bfloat16, device=dout.device)
-            ops._count(1)
-            check(lib().pnx_tap_scatter(ptr(dout), B, H, W, ptr(dZ), P * NZ, NZ, cpt, NZ, stream()))
+            dZ = ops.tap_scatter(dout, B, H, W, torch.empty(M, P * NZ, dtype=torch.bfloat16, device=dout.device), NZ, cpt, NZ)
             wzf = sum(wz[0, :, q * cin:(q + 1) * cin].float() for q in reversed(range(P)))  # [NZ, cin] (sum of the pieces)
             d32 = torch.empty(M, cin, dtype=torch.float32, device=dout.device)
             ops.igemm(dZ, M, _to_hilo(wzf.t().contiguous().unsqueeze(0)), 1, NZ, cin, d32, segs=ops.split_segments(), a_lo_off=NZ)
@@ -898,9 +871,7 @@ class HeadFinalConvFn(torch.autograd.Function):
             g = torch.zeros(1, cin, NZ, dtype=torch.float32, device=dout.device)
             ops.wgrad_split(y, cin, cin, dZ, NZ, NZ, M, 1, g)
             return dy, to_wb(g), dbias, None, None, None, None, None
-        dZ = torch.empty(M, NZ, dtype=torch.bfloat16, device=dout.device)
-        ops._count(1)
-        check(lib().pnx_tap_scatter(ptr(dout), B, H, W, ptr(dZ), NZ, NZ, cpt, 0, stream()))
+        dZ = ops.tap_scatter(dout, B, H, W, torch.empty(M, NZ, dtype=torch.bfloat16, device=dout.device), NZ, cpt)
         dy = torch.empty(M, cin, dtype=torch.bfloat16, device=dout.device)
         ops.igemm(dZ, M, wz.transpose(1, 2).contiguous(), 1, NZ, cin, dy,         # dy = dZ . Wz (+ the sibling BN's reduce pass)
                   bnr=_claim_bn_reduce(ctx.bn_src, M, cin, NZ))

@@ -238,14 +238,13 @@ class SparseResNet(nn.Module):
         dev = feat.device
         c = coors.to(dev).long()
         batch = int(c[:, 0].max().item()) + 1 if c.shape[0] else 1
-        L = ops.lib()
         vwords = (H + 31) // 32
         key = (c[:, 0] * W + c[:, 2]) * (vwords * 32) + c[:, 1]          # bit index: (b, x, y) order = the reader's sort order
         order = torch.argsort(key)
         key = key[order]
         if key.numel() > 1 and bool((key[1:] == key[:-1]).any()):
             raise ValueError("SparseResNet: duplicate (b, y, x) coordinates")
-        words = L.pnx_voxelize_bitmap_words(batch, W, H)
+        words = ops.bitmap_words(batch, W, H)
         bm = torch.zeros(words, dtype=torch.int32, device=dev)
         bits = torch.ones_like(key, dtype=torch.int32) << (key & 31).to(torch.int32)
         bm.index_add_(0, key >> 5, bits)                                   # distinct bits: the sum is the OR

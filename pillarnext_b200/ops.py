@@ -1,7 +1,11 @@
 """Thin host wrappers: torch device buffers + current stream -> libpnx C-ABI calls.
 
+This module is the only caller of libpnx: every entry point, including the host twins (`*_host`: the CPU builds of
+kernels, which take numpy arrays), is reached through a wrapper here.
 torch is used here for device memory, streams and dtype plumbing only; all compute is in libpnx.
 """
+import ctypes
+
 import numpy as np
 import torch
 
@@ -15,6 +19,30 @@ PROFILE = None          # when a list: (kind, flops, bytes, start_event, end_eve
 def _count(n):
     global LAUNCHES
     LAUNCHES += n
+
+
+# --------------------------------------------------------------------------------- operand checks
+_NUMPY = {torch.float32: np.dtype(np.float32), torch.float64: np.dtype(np.float64), torch.int32: np.dtype(np.int32),
+          torch.int64: np.dtype(np.int64)}
+
+
+def _want(t, dtype, shape, what, host=False):
+    """Check one operand of a libpnx call and return it C-contiguous.  A device entry point takes a CUDA tensor of
+    `dtype`; a host twin (host=True) takes a numpy array of the same element type.  A wrong dtype or shape raises here
+    instead of being read as garbage by the library."""
+    if host:
+        ok, kind = isinstance(t, np.ndarray) and t.dtype == _NUMPY[dtype], "a numpy %s array" % _NUMPY[dtype]
+    else:
+        ok, kind = isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype, "a CUDA %s tensor" % dtype
+    if not ok or tuple(t.shape) != tuple(shape):
+        raise ValueError("%s must be %s of shape %s, got %s %s %s" % (what, kind, tuple(shape), type(t).__name__,
+                                                                    getattr(t, "dtype", None), tuple(getattr(t, "shape", ()))))
+    return np.ascontiguousarray(t) if host else t.contiguous()
+
+
+def _hp(a):
+    """Address of a host twin's operand (a C-contiguous numpy array)."""
+    return a.ctypes.data
 
 
 class _Timed:
@@ -121,6 +149,16 @@ class Voxels:
 FRAME_TILED_MIN_CTAS = None
 
 
+def bitmap_words(batch, gx, gy):
+    """Words of the occupancy bitmap of a batch x gx x gy grid, padded to whole 32-word blocks (pnx_voxelize_bitmap_words)."""
+    return lib().pnx_voxelize_bitmap_words(batch, gx, gy)
+
+
+def voxelize_frames_supported(batch, gx, gy):
+    """CTAs the frame-tiled voxelizer (pnx_voxelize_frames) would launch for this geometry; 0 = not supported."""
+    return lib().pnx_voxelize_frames_supported(batch, gx, gy)
+
+
 def voxelize(points, batch, voxel_size, pc_range, buckets=True, frame_sorted=False):
     """V1-V2 index generation (pnx_voxelize) and, with buckets=True, the CSR grouping the PFN needs
     (pnx_bucketize). points [N,6] fp32 cuda (b,x,y,z,i,t).
@@ -139,7 +177,7 @@ def voxelize(points, batch, voxel_size, pc_range, buckets=True, frame_sorted=Fal
     gx, gy = int(g[0]), int(g[1])
     dev = points.device
     L = lib()
-    words = L.pnx_voxelize_bitmap_words(batch, gx, gy)
+    words = bitmap_words(batch, gx, gy)
     cap_p = min(n, batch * gx * gy)
     v = Voxels()
     v.points, v.n, v.batch, v.gx, v.gy, v.cap_p = points, n, batch, gx, gy, cap_p
@@ -156,7 +194,7 @@ def voxelize(points, batch, voxel_size, pc_range, buckets=True, frame_sorted=Fal
     bucket_cnt = torch.empty(2 * (cap_p + 1), **i32) if buckets else None
     v.counts = torch.zeros(2, **i32)
     v.status = None
-    n_cta = L.pnx_voxelize_frames_supported(batch, gx, gy) if (frame_sorted and n > 0) else 0
+    n_cta = voxelize_frames_supported(batch, gx, gy) if (frame_sorted and n > 0) else 0
     if n_cta > 0 and (frame_sorted == "force" or (FRAME_TILED_MIN_CTAS is not None and n_cta >= FRAME_TILED_MIN_CTAS)):
         scratch = torch.empty(L.pnx_voxelize_frames_scratch(batch), **i32)
         v.status = scratch[0:1]
@@ -353,7 +391,8 @@ def level_from_mask_words(bm, batch, U, V):
     _count(1)
     check(lib().pnx_sites_inblock(ptr(bm), bm.numel(), ptr(inblk), stream()))
     cnt = torch.zeros(lib().pnx_blockcnt_size(blocks), dtype=torch.int32, device=bm.device)
-    # block counts = in-block prefix of the last word + its popcount (host-side torch plumbing; test helper only)
+    # block counts = in-block prefix of the last word + its popcount (host-side torch plumbing, used by tests and by
+    # modules.SparseResNet for coordinates that do not come from the voxelizer)
     w = bm.view(-1, 32)
     pc = torch.zeros_like(w)
     x = w.clone().to(torch.int64) & 0xFFFFFFFF
@@ -519,6 +558,11 @@ def set_deterministic(on):
     return prev
 
 
+def wgrad_splits(x_channels, y_channels, taps, M, sms=None):
+    """Number of K splits pnx_wgrad uses for the shape (a pure function of it; sms defaults to this device's SM count)."""
+    return lib().pnx_wgrad_splits(x_channels, y_channels, taps, M, sm_count() if sms is None else sms)
+
+
 def wgrad(X, x_channels, Y, y_channels, M, taps, dW, *, nbr=None, dense=None, shuffle=False, gathered=None):
     """dW[t, x, y] += sum_m X[m, x] * Y[g(m,t), y]; X direct, Y gathered; dW fp32 [taps, x_channels, y_channels]."""
     assert X.dtype == torch.bfloat16 and Y.dtype == torch.bfloat16 and dW.dtype == torch.float32
@@ -537,7 +581,7 @@ def wgrad(X, x_channels, Y, y_channels, M, taps, dW, *, nbr=None, dense=None, sh
     if gathered is None:
         gathered = nbr is not None or dense is not None or shuffle
     # one slab per K split, added in split order (not fp32 atomics): the weight gradient is the same from run to run
-    splits = lib().pnx_wgrad_splits(x_channels, y_channels, taps, M, sm_count())
+    splits = wgrad_splits(x_channels, y_channels, taps, M)
     partials = torch.empty(max(splits, 1) * taps * x_channels * y_channels, dtype=torch.float32, device=dW.device)
     _count(2)
     with _Timed("wgrad", 2.0 * M * taps * x_channels * y_channels, 2.0 * M * (x_channels + taps * y_channels),
@@ -556,28 +600,42 @@ def bn_apply(x, M, C, scale, shift, y, res=None, relu=True):
     return y
 
 
-def bn_bwd(dy, y, x, M, C, mean, invstd, gamma, count, relu, dx, dres=None, dres_accumulate=False, affine=None, red=None):
-    """Returns red (fp64 [2C]: sum g = dbeta, sum g*xhat = dgamma); writes dx (and dres).
-    y=None (no residual): the ReLU mask is recomputed from x with affine=(scale, shift) of the forward.
-    red given: the reduce pass already happened in the epilogue of the GEMM that produced dy (which is then the gated
-    g, so the apply pass runs without a ReLU mask)."""
-    L = lib()
-    fs, fh = (affine if affine is not None else (None, None))
-    yp, ys = (ptr(y), y.stride(0)) if y is not None else (None, 8)
+def bn_bwd_reduce(dy, y, x, M, C, mean, invstd, relu, affine=None, red=None):
+    """Reduce pass of the BatchNorm backward (pnx_bn_bwd_reduce) -> red fp64 [2C] (sum g = dbeta, sum g*xhat = dgamma)
+    of the gated gradient g, added into `red` (default: a zeroed buffer of the step's arena).  y=None (no residual): the
+    ReLU mask is recomputed from x with affine=(scale, shift) of the forward."""
+    fs, fh = affine if affine is not None else (None, None)
     if red is None:
         red = zeros(2 * C, torch.float64, dy.device)
-        _count(1)
-        check(L.pnx_bn_bwd_reduce(ptr(dy), dy.stride(0), yp, ys, ptr(x), x.stride(0), M, C, ptr(mean), ptr(invstd),
-                                  1 if relu else 0, ptr(fs) if fs is not None else None, ptr(fh) if fh is not None else None,
-                                  ptr(red), stream()))
+    _count(1)
+    check(lib().pnx_bn_bwd_reduce(ptr(dy), dy.stride(0), ptr(y), y.stride(0) if y is not None else 8, ptr(x), x.stride(0),
+                                  M, C, ptr(mean), ptr(invstd), 1 if relu else 0, ptr(fs), ptr(fh), ptr(red), stream()))
+    return red
+
+
+def bn_bwd_apply(dy, y, x, M, C, mean, invstd, gamma, red, count, relu, affine, dx, dres=None, dres_accumulate=False,
+                 count_dev=None):
+    """Apply pass of the BatchNorm backward (pnx_bn_bwd_apply): writes dx (and dres) from the sums red of the reduce
+    pass.  relu=False when dy already is the gated g (the reduce pass ran in the epilogue of the GEMM that produced it).
+    count_dev: the population as a device int32 [1] (SyncBatchNorm), used instead of the host count."""
+    fs, fh = affine if affine is not None else (None, None)
+    _count(1)
+    check(lib().pnx_bn_bwd_apply(ptr(dy), dy.stride(0), ptr(y), y.stride(0) if y is not None else 8, ptr(x), x.stride(0),
+                                 M, C, ptr(mean), ptr(invstd), ptr(gamma), ptr(red), float(max(count, 1)), ptr(count_dev),
+                                 1 if relu else 0, ptr(fs), ptr(fh), ptr(dx), dx.stride(0), ptr(dres),
+                                 dres.stride(0) if dres is not None else 8, 1 if dres_accumulate else 0, stream()))
+    return dx
+
+
+def bn_bwd(dy, y, x, M, C, mean, invstd, gamma, count, relu, dx, dres=None, dres_accumulate=False, affine=None, red=None):
+    """Both passes of the BatchNorm backward: bn_bwd_reduce, then bn_bwd_apply with the host count.  Returns red.
+    red given: the reduce pass already happened in the epilogue of the GEMM that produced dy (which is then the gated
+    g, so the apply pass runs without a ReLU mask)."""
+    if red is None:
+        red = bn_bwd_reduce(dy, y, x, M, C, mean, invstd, relu, affine)
     else:
         relu = False
-    _count(1)
-    check(L.pnx_bn_bwd_apply(ptr(dy), dy.stride(0), yp, ys, ptr(x), x.stride(0), M, C, ptr(mean), ptr(invstd),
-                             ptr(gamma), ptr(red), float(max(count, 1)), None, 1 if relu else 0,
-                             ptr(fs) if fs is not None else None, ptr(fh) if fh is not None else None, ptr(dx),
-                             dx.stride(0), ptr(dres) if dres is not None else None,
-                             dres.stride(0) if dres is not None else 8, 1 if dres_accumulate else 0, stream()))
+    bn_bwd_apply(dy, y, x, M, C, mean, invstd, gamma, red, count, relu, affine, dx, dres=dres, dres_accumulate=dres_accumulate)
     return red
 
 
@@ -706,6 +764,47 @@ def wgrad_split(X, x_lo, x_channels, Y, y_lo, y_channels, M, taps, dW, **kw):
     return dW
 
 
+# --------------------------------------------------------------------------------- head final convs: 9-tap stencil
+def tap_gather_sum(Z, cpt, bias, B, H, W, out):
+    """out [B*H*W, 16] fp32 = bias + the sum over the 9 taps of the stencil of Z [B*H*W, >= 9*cpt] fp32, column
+    tap*cpt + j (pnx_tap_gather_sum)."""
+    _count(1)
+    check(lib().pnx_tap_gather_sum(ptr(Z), Z.stride(0), cpt, ptr(bias), B, H, W, ptr(out), stream()))
+    return out
+
+
+def tap_scatter(dout, B, H, W, dZ, nz, cpt, lo_off=0):
+    """Backward of tap_gather_sum (pnx_tap_scatter): dZ [B*H*W, nz] bf16 (columns >= 9*cpt zeroed) from dout fp32;
+    lo_off > 0: all pieces of a split-rows dZ, piece q at column q*lo_off + c."""
+    _count(1)
+    check(lib().pnx_tap_scatter(ptr(dout), B, H, W, ptr(dZ), dZ.stride(0), nz, cpt, lo_off, stream()))
+    return dZ
+
+
+# --------------------------------------------------------------------------------- L1: fused CenterPoint loss
+def center_loss_task(out, dout, labels, task, weight, code_weights, with_iou, acc):
+    """Loss partial sums of one task into acc fp64 [16] (zeroed) and the gradient dout (pnx_center_loss_task).
+    out/dout [B*H*W, npad] fp32; labels: the task's hm / anno_box / ind / mask / cat / gt_boxes (assign_labels);
+    task: its geometry B, H, W, npad, C, M, column offsets `off` and the sx, sy, ox, oy of the box encoding."""
+    cw, cwp = _host_floats(code_weights, 10)
+    o = task["off"]
+    _count(2)
+    check(lib().pnx_center_loss_task(ptr(out), ptr(dout), ptr(labels["hm"]), ptr(labels["anno_box"]), ptr(labels["ind"]),
+                                     ptr(labels["mask"]), ptr(labels["cat"]), ptr(labels["gt_boxes"]), task["B"], task["H"],
+                                     task["W"], task["npad"], task["C"], task["M"], o["reg"], o["height"], o["dim"], o["rot"],
+                                     o["vel"], o["hm"], task["sx"], task["sy"], task["ox"], task["oy"], weight, cwp,
+                                     1 if with_iou else 0, ptr(acc), stream()))
+    return dout
+
+
+def center_loss_finalize(acc, weights_dev, code_w_dev, with_iou_dev, res, total):
+    """acc [T, 16] fp64 of center_loss_task -> res [T, 16] per-task losses and total [1] (pnx_center_loss_finalize)."""
+    _count(1)
+    check(lib().pnx_center_loss_finalize(ptr(acc), acc.shape[0], ptr(weights_dev), ptr(code_w_dev), ptr(with_iou_dev),
+                                         ptr(res), ptr(total), stream()))
+    return res, total
+
+
 # --------------------------------------------------------------------------------- F3: label assignment
 _cls_tables = {}
 
@@ -757,9 +856,18 @@ def assign_labels(gt_boxes, gt_cls, tasks, voxel_size, pc_range, out_size_factor
 
 # --------------------------------------------------------------------------------- F1: decode + rotated NMS
 def _host_floats(vals, n):
-    import ctypes
     a = (ctypes.c_float * n)(*([float(v) for v in vals] + [0.0] * (n - len(vals))))
     return a, ctypes.addressof(a)
+
+
+def _decode_params(offs, osf, voxel_size, pc_range, score_thr, post_center_range, rectifier):
+    """The decode parameters of the F1 entry points and their host twins, after (out, ld, B, H, W, C): -> (the host
+    arrays they point to, to be kept alive across the calls; the arguments)."""
+    offs_a = (ctypes.c_int * 7)(*[int(o) for o in offs])
+    r6, r6p = _host_floats(post_center_range, 6)
+    rc, rcp = _host_floats(rectifier, 8)
+    return (offs_a, r6, rc), (ctypes.addressof(offs_a), float(osf), float(voxel_size[0]), float(voxel_size[1]),
+                              float(pc_range[0]), float(pc_range[1]), float(score_thr), r6p, rcp)
 
 
 def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr, post_center_range, rectifier, nms_thr,
@@ -772,16 +880,12 @@ def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr,
     double_flip=True: `out` is the head output of a flip4_points batch, [4B*H*W, ld] (frame 4b + k = copy k of frame b);
     the decode merges the four copies of each pixel (pnx_det_*_flip4, include/pnx.h) and the results are those of the
     B original frames."""
-    import ctypes
     assert out.dtype == torch.float32 and out.is_cuda and out.dim() == 2 and out.shape[0] == (4 if double_flip else 1) * B * H * W
     dev = out.device
     M, nseg = B * H * W, B * C
-    offs_a = (ctypes.c_int * 7)(*[int(o) for o in offs])
-    r6, r6p = _host_floats(post_center_range, 6)
-    rc, rcp = _host_floats(rectifier, 8)
+    alive, params = _decode_params(offs, osf, voxel_size, pc_range, score_thr, post_center_range, rectifier)
     nt, ntp = _host_floats(nms_thr, 8)
-    common = (ptr(out), out.stride(0), B, H, W, C, ctypes.addressof(offs_a), float(osf), float(voxel_size[0]),
-              float(voxel_size[1]), float(pc_range[0]), float(pc_range[1]), float(score_thr), r6p, rcp)
+    common = (ptr(out), out.stride(0), B, H, W, C) + params
     keys = torch.empty(M, dtype=torch.int64, device=dev)
     seg_count = torch.empty(nseg, dtype=torch.int32, device=dev)
     L = lib()
@@ -807,6 +911,42 @@ def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr,
     return det_box, det_score, det_label, keep_count
 
 
+def det_decode_host(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr, post_center_range, rectifier,
+                    double_flip=False):
+    """Host twin of the decode of det_postprocess (pnx_det_decode_host, pnx_det_decode_flip4_host with double_flip):
+    `out` numpy fp32 [B*H*W (4B*H*W with double_flip), ld] -> keep [B*H*W] bool (score above the threshold and centre in
+    post_center_range), box [B*H*W, 9] fp32, score fp32, label int32 (meaningful where keep) of every output pixel."""
+    need = max(offs[0] + 2, offs[1] + 1, offs[2] + 3, offs[3] + 2, offs[4] + 2, offs[5] + C, offs[6] + 1)
+    ld = out.shape[1] if out.ndim == 2 else 0
+    if ld < need:
+        raise ValueError("out must have at least %d columns for these offsets, got shape %s" % (need, out.shape))
+    M = B * H * W
+    out = _want(out, torch.float32, ((4 if double_flip else 1) * M, ld), "out", host=True)
+    alive, params = _decode_params(offs, osf, voxel_size, pc_range, score_thr, post_center_range, rectifier)
+    keep = np.zeros(M, bool)
+    box, score, label = np.zeros((M, 9), np.float32), np.zeros(M, np.float32), np.zeros(M, np.int32)
+    fn = lib().pnx_det_decode_flip4_host if double_flip else lib().pnx_det_decode_host
+    for m in range(M):
+        rc = fn(_hp(out), ld, B, H, W, C, *params, m, _hp(box[m]), _hp(score[m:]), _hp(label[m:]))
+        if rc < 0:
+            check(rc)
+        keep[m] = rc == 1
+    return keep, box, score, label
+
+
+def det_iou_bev_host(a, b):
+    """Rotated bird's-eye-view IoU of the NMS (pnx_det_iou_bev_host) of each pair a[i], b[i]: numpy fp32 [n, 7]
+    (x, y, z, dx, dy, dz, heading) -> [n] fp32."""
+    return _box_pairs_host(lib().pnx_det_iou_bev_host, a, b)
+
+
+def _box_pairs_host(fn, a, b):
+    """fn(box7_a, box7_b) -> float of a host twin on each pair of rows of a, b (numpy fp32 [n, 7]) -> [n] fp32."""
+    n = len(a)
+    a, b = _want(a, torch.float32, (n, 7), "a", host=True), _want(b, torch.float32, (n, 7), "b", host=True)
+    return np.array([fn(_hp(a[i]), _hp(b[i])) for i in range(n)], np.float32)
+
+
 def flip4_points(points):
     """Double-flip test-time augmentation: points [N, 6] (b, x, y, z, i, t) fp32 cuda -> [4N, 6], copy k of point i at row
     k*N + i in frame 4b + k (k = 1: y -> -y, k = 2: x -> -x, k = 3: both; pnx_flip4_points).  The rows are NOT grouped by
@@ -820,24 +960,47 @@ def flip4_points(points):
     return out
 
 
+def _global_aug_operands(points, gt_boxes, aug, host=False):
+    B, M = gt_boxes.shape[:2] if gt_boxes.ndim == 3 else (0, 0)
+    return (_want(points, torch.float32, (len(points), 6), "points (batch_idx, x, y, z, intensity, time)", host),
+            _want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes", host),
+            _want(aug, torch.float64, (B, 4, 4), "aug", host))
+
+
 def global_aug(points, gt_boxes, aug):
     """Global training augmentation on the GPU (pnx_global_aug, include/pnx.h): points [N, 6] (b, x, y, z, i, t) fp32
     cuda, raw boxes [B, M, 9] fp32 cuda and the collated records aug [B, 4, 4] fp64 cuda (det3d.datasets.pipelines.
     augmentation) -> (points, boxes), new tensors with the reference's numpy results to the bit.  The inputs are left
     untouched and the point order is kept, so frame-sorted points stay frame-sorted."""
-    assert points.is_cuda and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 6, \
-        "points must be a CUDA float32 [N, 6] tensor (batch_idx, x, y, z, intensity, time)"
-    assert gt_boxes.is_cuda and gt_boxes.dtype == torch.float32 and gt_boxes.dim() == 3 and gt_boxes.shape[2] == 9, \
-        "gt_boxes must be a CUDA float32 [B, M, 9] tensor"
-    assert aug.is_cuda and aug.dtype == torch.float64 and tuple(aug.shape) == (gt_boxes.shape[0], 4, 4), \
-        "aug must be a CUDA float64 [B, 4, 4] tensor (B = gt_boxes.shape[0])"
-    points, gt_boxes, aug = points.contiguous(), gt_boxes.contiguous(), aug.contiguous()
+    points, gt_boxes, aug = _global_aug_operands(points, gt_boxes, aug)
     pts_out, box_out = torch.empty_like(points), torch.empty_like(gt_boxes)
     B, M = gt_boxes.shape[:2]
     _count(1)
     check(lib().pnx_global_aug(ptr(points), points.shape[0], ptr(gt_boxes), B, M, ptr(aug), ptr(pts_out), ptr(box_out),
                                stream()))
     return pts_out, box_out
+
+
+def global_aug_host(points, gt_boxes, aug):
+    """Host twin of global_aug (pnx_global_aug_host): the same operands as numpy arrays -> (points, boxes), new arrays."""
+    points, gt_boxes, aug = _global_aug_operands(points, gt_boxes, aug, host=True)
+    pts_out, box_out = np.empty_like(points), np.empty_like(gt_boxes)
+    B, M = gt_boxes.shape[:2]
+    check(lib().pnx_global_aug_host(_hp(points), len(points), _hp(gt_boxes), B, M, _hp(aug), _hp(pts_out), _hp(box_out)))
+    return pts_out, box_out
+
+
+def _gt_sample_operands(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, cand_trig, cand_points,
+                        cand_offsets, host=False):
+    B, M = gt_boxes.shape[:2] if gt_boxes.ndim == 3 else (0, 0)
+    S = cand_boxes.shape[1] if cand_boxes.ndim == 3 else 0
+    f32, i32 = torch.float32, torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (points, f32, (len(points), 6), "points"), (gt_boxes, f32, (B, M, 9), "gt_boxes"),
+        (gt_classes, i32, (B, M), "gt_classes"), (gt_trig, f32, (B, M, 2), "gt_trig"),
+        (cand_boxes, f32, (B, S, 9), "cand_boxes"), (cand_classes, i32, (B, S), "cand_classes"),
+        (cand_trig, f32, (B, S, 4), "cand_trig"), (cand_points, f32, (len(cand_points), 5), "cand_points"),
+        (cand_offsets, i32, (B * S + 1,), "cand_offsets"))]
 
 
 def gt_sample(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, cand_trig, cand_points, cand_offsets):
@@ -848,35 +1011,55 @@ def gt_sample(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, c
     (points [N + P, 6], boxes [B, M + S, 9], classes [B, M + S] int32, accepted [B, S] int32, count [1] int32 cuda).
     The rows past `count` have batch index B, which the voxelizers drop; the host does not wait for the count.  Frames
     stay in order, each with its pasted objects' points first, so frame-sorted input stays frame-sorted."""
-    def want(t, dtype, shape, what):
-        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
-            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
-    assert points.dim() == 2 and gt_boxes.dim() == 3 and cand_boxes.dim() == 3, "points [N, 6], boxes [B, M, 9], [B, S, 9]"
-    (n, _), (B, M, _), S = points.shape, gt_boxes.shape, cand_boxes.shape[1]
-    P = cand_points.shape[0]
-    want(points, torch.float32, (n, 6), "points")
-    want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes")
-    want(gt_classes, torch.int32, (B, M), "gt_classes")
-    want(gt_trig, torch.float32, (B, M, 2), "gt_trig")
-    want(cand_boxes, torch.float32, (B, S, 9), "cand_boxes")
-    want(cand_classes, torch.int32, (B, S), "cand_classes")
-    want(cand_trig, torch.float32, (B, S, 4), "cand_trig")
-    want(cand_points, torch.float32, (P, 5), "cand_points")
-    want(cand_offsets, torch.int32, (B * S + 1,), "cand_offsets")
-    args = [t.contiguous() for t in (points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, cand_trig,
-                                     cand_points, cand_offsets)]
-    dev = points.device
+    p, b, c, t, cb, cc, ct, cp, co = _gt_sample_operands(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes,
+                                                         cand_trig, cand_points, cand_offsets)
+    n, (B, M), S, P = len(p), b.shape[:2], cb.shape[1], len(cp)
+    dev = p.device
     pts_out = torch.empty((n + P, 6), dtype=torch.float32, device=dev)
     box_out = torch.empty((B, M + S, 9), dtype=torch.float32, device=dev)
     cls_out = torch.empty((B, M + S), dtype=torch.int32, device=dev)
     accepted = torch.empty((B, S), dtype=torch.int32, device=dev)
     count = torch.empty(1, dtype=torch.int32, device=dev)
     ws = torch.empty(max(4, lib().pnx_gt_sample_workspace(n, B, S)), dtype=torch.uint8, device=dev)
-    p, b, c, t, cb, cc, ct, cp, co = args
     _count(1)
     check(lib().pnx_gt_sample(ptr(p), n, ptr(b), ptr(c), ptr(t), B, M, ptr(cb), ptr(cc), ptr(ct), S, ptr(cp), ptr(co), P,
                               ptr(pts_out), ptr(box_out), ptr(cls_out), ptr(accepted), ptr(count), ptr(ws), stream()))
     return pts_out, box_out, cls_out, accepted, count
+
+
+def gt_sample_host(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes, cand_trig, cand_points, cand_offsets):
+    """Host twin of gt_sample (pnx_gt_sample_host): the same operands as numpy arrays -> (points, boxes, classes,
+    accepted, count), the first four new arrays and count an int."""
+    p, b, c, t, cb, cc, ct, cp, co = _gt_sample_operands(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_classes,
+                                                         cand_trig, cand_points, cand_offsets, host=True)
+    n, (B, M), S, P = len(p), b.shape[:2], cb.shape[1], len(cp)
+    pts_out = np.full((n + P, 6), np.nan, np.float32)          # every row is written: a NaN left over is a twin's bug
+    box_out, cls_out = np.zeros((B, M + S, 9), np.float32), np.zeros((B, M + S), np.int32)
+    accepted, count = np.zeros((B, S), np.int32), np.zeros(1, np.int32)
+    check(lib().pnx_gt_sample_host(_hp(p), n, _hp(b), _hp(c), _hp(t), B, M, _hp(cb), _hp(cc), _hp(ct), S, _hp(cp), _hp(co),
+                                   P, _hp(pts_out), _hp(box_out), _hp(cls_out), _hp(accepted), _hp(count)))
+    return pts_out, box_out, cls_out, accepted, int(count[0])
+
+
+def _row_shape(t, min_cols, what):
+    """Shape (n, c) of a [n, >= min_cols] operand; raises otherwise."""
+    shape = tuple(getattr(t, "shape", ()))
+    if len(shape) != 2 or shape[1] < min_cols:
+        raise ValueError("%s must be [n, >= %d], got shape %s" % (what, min_cols, shape))
+    return shape
+
+
+def points_in_boxes_host(points, boxes, trig):
+    """The point test of gt_sample on the host (pnx_points_in_boxes_host, the reference's points_in_rbbox): points numpy
+    fp32 [n, >= 3] (x, y, z first), boxes [m, 9] fp32, trig [m, 2] fp32 = libm (cosf, sinf) of each yaw -> inside
+    [n, m] bool."""
+    points = _want(points, torch.float32, _row_shape(points, 3, "points"), "points", host=True)
+    m = len(boxes)
+    boxes = _want(boxes, torch.float32, (m, 9), "boxes", host=True)
+    trig = _want(trig, torch.float32, (m, 2), "trig", host=True)
+    inside = np.zeros((len(points), m), np.uint8)
+    check(lib().pnx_points_in_boxes_host(_hp(points), len(points), points.shape[1], _hp(boxes), _hp(trig), m, _hp(inside)))
+    return inside.astype(bool)
 
 
 def aligned_iou3d(boxes_a, boxes_b):
@@ -889,28 +1072,56 @@ def aligned_iou3d(boxes_a, boxes_b):
     return out
 
 
+def aligned_iou3d_host(a, b):
+    """Host twin of aligned_iou3d (pnx_aligned_iou3d_host): numpy fp32 [n, 7] x [n, 7] -> [n] fp32."""
+    return _box_pairs_host(lib().pnx_aligned_iou3d_host, a, b)
+
+
 # --------------------------------------------------------------------------------- Waymo-style evaluation
+def _count_points_operands(boxes, classes, trig, host=False):
+    B, M = boxes.shape[:2] if boxes.ndim == 3 else (0, 0)
+    return (_want(boxes, torch.float32, (B, M, 9), "boxes", host), _want(classes, torch.int32, (B, M), "classes", host),
+            _want(trig, torch.float32, (B, M, 2), "trig", host))
+
+
 def eval_count_points(points, boxes, classes, trig):
     """Points inside each ground-truth box (pnx_eval_count_points, include/pnx.h), with the reference's
     points_in_boxes_jit test: points [N, >= 4] fp32 (batch_idx, x, y, z, ...), boxes [B, M, 9] fp32, classes [B, M]
     int32 (-1 = padding), trig [B, M, 2] fp32 libm (cosf, sinf) of each yaw, all CUDA -> counts [B, M] int32 cuda."""
-    def want(t, dtype, shape, what):
-        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
-            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
-    assert points.dim() == 2 and points.shape[1] >= 4 and boxes.dim() == 3, "points [N, >= 4], boxes [B, M, 9]"
-    B, M = boxes.shape[:2]
-    want(points, torch.float32, points.shape, "points")
-    want(boxes, torch.float32, (B, M, 9), "boxes")
-    want(classes, torch.int32, (B, M), "classes")
-    want(trig, torch.float32, (B, M, 2), "trig")
+    _want(points, torch.float32, _row_shape(points, 4, "points"), "points")
     points = points if points.stride(1) == 1 else points.contiguous()
     row = points.stride(0) if points.shape[0] > 1 else points.shape[1]    # an empty or one-row tensor's stride is arbitrary
-    boxes, classes, trig = boxes.contiguous(), classes.contiguous(), trig.contiguous()
+    boxes, classes, trig = _count_points_operands(boxes, classes, trig)
+    B, M = classes.shape
     counts = torch.empty((B, M), dtype=torch.int32, device=boxes.device)
     _count(1)
     check(lib().pnx_eval_count_points(ptr(points), points.shape[0], row, ptr(boxes), ptr(classes), ptr(trig), B, M,
                                       ptr(counts), stream()))
     return counts
+
+
+def eval_count_points_host(points, boxes, classes, trig):
+    """Host twin of eval_count_points (pnx_eval_count_points_host): the same operands as numpy arrays -> counts [B, M]
+    int32."""
+    points = _want(points, torch.float32, _row_shape(points, 4, "points"), "points", host=True)
+    boxes, classes, trig = _count_points_operands(boxes, classes, trig, host=True)
+    B, M = classes.shape
+    counts = np.zeros((B, M), np.int32)
+    check(lib().pnx_eval_count_points_host(_hp(points), len(points), points.shape[1], _hp(boxes), _hp(classes), _hp(trig),
+                                           B, M, _hp(counts)))
+    return counts
+
+
+def _eval_match_operands(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, thresholds,
+                         host=False):
+    D, C = len(det_boxes), len(thresholds)
+    B, M = gt_boxes.shape[:2] if gt_boxes.ndim == 3 else (0, 0)
+    f32, i32 = torch.float32, torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (det_boxes, f32, (D, 9), "det_boxes"), (det_trig, f32, (D, 2), "det_trig"), (order, torch.int64, (D,), "order"),
+        (seg_start, i32, (B * C,), "seg_start"), (seg_count, i32, (B * C,), "seg_count"),
+        (gt_boxes, f32, (B, M, 9), "gt_boxes"), (gt_classes, i32, (B, M), "gt_classes"),
+        (gt_trig, f32, (B, M, 2), "gt_trig"), (thresholds, f32, (C,), "thresholds"))]
 
 
 def eval_match(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, thresholds):
@@ -919,24 +1130,10 @@ def eval_match(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_cl
     f C + c, then descending score, ties by lower index), seg_start / seg_count [B C] int32, gt_boxes [B, M, 9] fp32,
     gt_classes [B, M] int32 (-1 = padding), gt_trig [B, M, 2] fp32, thresholds [C] fp32 ->
     (match [D] int32 box index within the frame or -1, iou [D] fp32, heading accuracy [D] fp32)."""
-    def want(t, dtype, shape, what):
-        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
-            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
-    assert det_boxes.dim() == 2 and gt_boxes.dim() == 3 and thresholds.dim() == 1, "det_boxes [D, 9], gt_boxes [B, M, 9]"
-    D, (B, M), C = det_boxes.shape[0], gt_boxes.shape[:2], thresholds.shape[0]
-    want(det_boxes, torch.float32, (D, 9), "det_boxes")
-    want(det_trig, torch.float32, (D, 2), "det_trig")
-    want(order, torch.int64, (D,), "order")
-    want(seg_start, torch.int32, (B * C,), "seg_start")
-    want(seg_count, torch.int32, (B * C,), "seg_count")
-    want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes")
-    want(gt_classes, torch.int32, (B, M), "gt_classes")
-    want(gt_trig, torch.float32, (B, M, 2), "gt_trig")
-    want(thresholds, torch.float32, (C,), "thresholds")
-    args = [t.contiguous() for t in (det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig,
-                                     thresholds)]
-    db, dt, od, ss, sc, gb, gc, gt, th = args
-    dev = det_boxes.device
+    db, dt, od, ss, sc, gb, gc, gt, th = _eval_match_operands(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes,
+                                                              gt_classes, gt_trig, thresholds)
+    D, (B, M), C = len(db), gb.shape[:2], len(th)
+    dev = db.device
     match = torch.empty(D, dtype=torch.int32, device=dev)
     iou = torch.empty(D, dtype=torch.float32, device=dev)
     heading = torch.empty(D, dtype=torch.float32, device=dev)
@@ -946,29 +1143,53 @@ def eval_match(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_cl
     return match, iou, heading
 
 
+def eval_match_host(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, thresholds):
+    """Host twin of eval_match (pnx_eval_match_host): the same operands as numpy arrays -> (match, iou, heading)."""
+    db, dt, od, ss, sc, gb, gc, gt, th = _eval_match_operands(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes,
+                                                              gt_classes, gt_trig, thresholds, host=True)
+    D, (B, M), C = len(db), gb.shape[:2], len(th)
+    match, iou, heading = np.zeros(D, np.int32), np.zeros(D, np.float32), np.zeros(D, np.float32)
+    check(lib().pnx_eval_match_host(_hp(db), _hp(dt), D, _hp(od), _hp(ss), _hp(sc), _hp(gb), _hp(gc), _hp(gt), B, M, C,
+                                    _hp(th), _hp(match), _hp(iou), _hp(heading)))
+    return match, iou, heading
+
+
 # --------------------------------------------------------------------------------- nuScenes detection score
+def _eval_match_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, dist_ths,
+                                host=False):
+    D, T, C = len(det_boxes), len(dist_ths), int(n_classes)
+    B, M = gt_boxes.shape[:2] if gt_boxes.ndim == 3 else (0, 0)
+    f32, i32 = torch.float32, torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (det_boxes, f32, (D, 9), "det_boxes"), (order, torch.int64, (D,), "order"),
+        (seg_start, i32, (B * C,), "seg_start"), (seg_count, i32, (B * C,), "seg_count"),
+        (gt_boxes, f32, (B, M, 9), "gt_boxes"), (gt_classes, i32, (B, M), "gt_classes"),
+        (dist_ths, torch.float64, (T,), "dist_ths"))]
+
+
 def eval_match_center(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, dist_ths):
     """Centre-distance matching per (frame, class) segment and distance threshold (pnx_eval_match_center,
     include/pnx.h), all CUDA: det_boxes [D, 9] fp32, order [D] int64 (detections sorted by segment f C + c, then in
     visit order), seg_start / seg_count [B C] int32, gt_boxes [B, M, 9] fp32, gt_classes [B, M] int32 in [0, C) (-1 =
     padding or filtered out), C = n_classes, dist_ths [T] fp64 -> match [T, D] int32, the box index within the frame
     or -1."""
-    def want(t, dtype, shape, what):
-        assert t.is_cuda and t.dtype == dtype and tuple(t.shape) == tuple(shape), \
-            "%s must be a CUDA %s tensor of shape %s, got %s %s" % (what, dtype, tuple(shape), t.dtype, tuple(t.shape))
-    assert det_boxes.dim() == 2 and gt_boxes.dim() == 3 and dist_ths.dim() == 1, "det_boxes [D, 9], gt_boxes [B, M, 9]"
-    D, (B, M), T, C = det_boxes.shape[0], gt_boxes.shape[:2], dist_ths.shape[0], int(n_classes)
-    want(det_boxes, torch.float32, (D, 9), "det_boxes")
-    want(order, torch.int64, (D,), "order")
-    want(seg_start, torch.int32, (B * C,), "seg_start")
-    want(seg_count, torch.int32, (B * C,), "seg_count")
-    want(gt_boxes, torch.float32, (B, M, 9), "gt_boxes")
-    want(gt_classes, torch.int32, (B, M), "gt_classes")
-    want(dist_ths, torch.float64, (T,), "dist_ths")
-    db, od, ss, sc, gb, gc, th = [t.contiguous() for t in (det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes,
-                                                            dist_ths)]
-    match = torch.empty((T, D), dtype=torch.int32, device=det_boxes.device)
+    db, od, ss, sc, gb, gc, th = _eval_match_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes,
+                                                             n_classes, dist_ths)
+    D, (B, M), T, C = len(db), gb.shape[:2], len(th), int(n_classes)
+    match = torch.empty((T, D), dtype=torch.int32, device=db.device)
     _count(1)
     check(lib().pnx_eval_match_center(ptr(db), D, ptr(od), ptr(ss), ptr(sc), ptr(gb), ptr(gc), B, M, C, ptr(th), T,
                                       ptr(match), stream()))
+    return match
+
+
+def eval_match_center_host(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, dist_ths):
+    """Host twin of eval_match_center (pnx_eval_match_center_host): the same operands as numpy arrays -> match [T, D]
+    int32."""
+    db, od, ss, sc, gb, gc, th = _eval_match_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes,
+                                                             n_classes, dist_ths, host=True)
+    D, (B, M), T, C = len(db), gb.shape[:2], len(th), int(n_classes)
+    match = np.zeros((T, D), np.int32)
+    check(lib().pnx_eval_match_center_host(_hp(db), D, _hp(od), _hp(ss), _hp(sc), _hp(gb), _hp(gc), B, M, C, _hp(th), T,
+                                           _hp(match)))
     return match

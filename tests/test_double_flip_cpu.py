@@ -6,7 +6,6 @@
 * the product's flip-merging decode, compiled for the host (pnx_det_decode_flip4_host), matches the oracle pixel by pixel;
 * the double-flip preconditions and the `+model.post_processing.double_flip=True` override.
 """
-import ctypes
 import math
 import os
 
@@ -82,8 +81,7 @@ def rows_with_iou(pd, with_iou):
 
 @pytest.mark.parametrize("with_iou,rect_v", [(False, [0.0, 0.0]), (True, [0.71, 0.65])])
 def test_host_compiled_flip_decode_matches_oracle(with_iou, rect_v):
-    from pillarnext_b200 import _lib
-    L = _lib.lib()
+    from pillarnext_b200 import ops
     cfg = _test_cfg()
     B, H, W, C = 2, 12, 10, 2
     pd = fake_preds(4 * B, H, W, C, 23)                         # four unrelated copies: every merge term matters
@@ -97,22 +95,17 @@ def test_host_compiled_flip_decode_matches_oracle(with_iou, rect_v):
     keep = (scores > cfg["score_threshold"]) & (boxes[..., :3] >= pcr[:3]).all(-1) & (boxes[..., :3] <= pcr[3:]).all(-1)
     rect = torch.tensor(rect_v)[labels]
     scores = torch.pow(scores, 1 - rect) * torch.pow(torch.clamp(iou, 0, 1), rect)
-    A = ctypes.addressof
-    offs_a = (ctypes.c_int * 7)(*offs)
-    r6 = (ctypes.c_float * 6)(*cfg["post_center_limit_range"])
-    rc8 = (ctypes.c_float * 8)(*(rect_v + [0.0] * 6))
-    b9, sc, lb = (ctypes.c_float * 9)(), ctypes.c_float(), ctypes.c_int()
+    kept, b9, sc, lb = ops.det_decode_host(out.numpy(), B, H, W, C, offs, 4.0, [0.075, 0.075], [-50.4, -50.4],
+                                           cfg["score_threshold"], cfg["post_center_limit_range"], rect_v, double_flip=True)
     n_kept = 0
     for m in range(B * H * W):
-        rc = L.pnx_det_decode_flip4_host(out.data_ptr(), out.stride(0), B, H, W, C, A(offs_a), 4.0, 0.075, 0.075, -50.4,
-                                         -50.4, cfg["score_threshold"], A(r6), A(rc8), m, A(b9), A(sc), A(lb))
         b, i = divmod(m, H * W)
-        assert rc == int(keep[b, i]), (m, rc)
-        if rc:
+        assert kept[m] == bool(keep[b, i]), (m, kept[m])
+        if kept[m]:
             n_kept += 1
-            assert lb.value == int(labels[b, i])
-            assert abs(sc.value - float(scores[b, i])) < 2e-6
-            assert torch.allclose(torch.tensor(list(b9)), boxes[b, i], atol=1e-5, rtol=1e-6)
+            assert lb[m] == int(labels[b, i])
+            assert abs(float(sc[m]) - float(scores[b, i])) < 2e-6
+            assert torch.allclose(torch.from_numpy(b9[m]), boxes[b, i], atol=1e-5, rtol=1e-6)
     assert 20 < n_kept < B * H * W and not keep[0, 0]
 
 

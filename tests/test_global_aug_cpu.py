@@ -40,14 +40,8 @@ def np_random_state():
 
 
 def host_aug(points, boxes, aug):
-    from pillarnext_b200 import _lib
-    points, boxes, aug = (np.ascontiguousarray(points, np.float32), np.ascontiguousarray(boxes, np.float32),
-                          np.ascontiguousarray(aug, np.float64))
-    p_out, b_out = np.empty_like(points), np.empty_like(boxes)
-    rc = _lib.lib().pnx_global_aug_host(points.ctypes.data, points.shape[0], boxes.ctypes.data, boxes.shape[0], boxes.shape[1],
-                                        aug.ctypes.data, p_out.ctypes.data, b_out.ctypes.data)
-    assert rc == 0
-    return p_out, b_out
+    from pillarnext_b200 import ops
+    return ops.global_aug_host(np.asarray(points, np.float32), np.asarray(boxes, np.float32), np.asarray(aug, np.float64))
 
 
 def test_dropin_classes_draw_the_reference_parameters(np_random_state, monkeypatch):

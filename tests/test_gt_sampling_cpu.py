@@ -94,20 +94,10 @@ def golden_expected(g):
 
 
 def host_gts(points, boxes, classes, trig, cboxes, cclasses, ctrig, cpoints, coffsets):
-    from pillarnext_b200 import _lib
-    c = lambda a, t: np.ascontiguousarray(a, t)
-    points, boxes, trig, cboxes, ctrig, cpoints = (c(a, np.float32) for a in (points, boxes, trig, cboxes, ctrig, cpoints))
-    classes, cclasses, coffsets = c(classes, np.int32), c(cclasses, np.int32), c(coffsets, np.int32)
-    (B, M, _), S, n, P = boxes.shape, cboxes.shape[1], points.shape[0], cpoints.shape[0]
-    p_out = np.full((n + P, 6), np.nan, np.float32)
-    b_out, c_out = np.zeros((B, M + S, 9), np.float32), np.zeros((B, M + S), np.int32)
-    acc, count = np.zeros((B, S), np.int32), np.zeros(1, np.int32)
-    rc = _lib.lib().pnx_gt_sample_host(points.ctypes.data, n, boxes.ctypes.data, classes.ctypes.data, trig.ctypes.data, B,
-                                       M, cboxes.ctypes.data, cclasses.ctypes.data, ctrig.ctypes.data, S,
-                                       cpoints.ctypes.data, coffsets.ctypes.data, P, p_out.ctypes.data, b_out.ctypes.data,
-                                       c_out.ctypes.data, acc.ctypes.data, count.ctypes.data)
-    assert rc == 0
-    return p_out, b_out, c_out, acc, int(count[0])
+    from pillarnext_b200 import ops
+    f, i = (lambda a: np.asarray(a, np.float32)), (lambda a: np.asarray(a, np.int32))
+    return ops.gt_sample_host(f(points), f(boxes), i(classes), f(trig), f(cboxes), i(cclasses), f(ctrig), f(cpoints),
+                              i(coffsets))
 
 
 def test_dropin_sampler_draws_the_reference_candidates(tmp_path, np_random_state):

@@ -4,13 +4,12 @@ itself pinned to the reference's predict and iou3d_cpu.cpp by tests/test_predict
 Scores/boxes are fp32 on both sides (tolerance 1e-5: expf/atan2f implementations differ in the last ulp); the kept SETS
 must be identical -- the inputs are screened so that no candidate pair sits within 1e-4 of the IoU threshold, where
 a last-ulp difference could legitimately flip a suppression decision."""
-import ctypes
-
+import numpy as np
 import pytest
 import torch
 
 from oracle import predict_oracle as P
-from pillarnext_b200 import _lib, modules, ops, synth
+from pillarnext_b200 import modules, ops, synth
 from oracle.predict_fixtures import fake_preds as _fake_preds, test_cfg as _test_cfg, to_rows
 
 pytestmark = pytest.mark.gpu
@@ -33,13 +32,9 @@ def clustered_preds(B, H, W, classes, seed, n=160):
 
 def screen(boxes7, thr, margin=1e-4):
     """True when no pair of candidate boxes has an IoU within `margin` of the threshold (host-compiled product IoU)."""
-    L = _lib.lib()
-    b = boxes7.contiguous().numpy()
-    for i in range(len(b)):
-        for j in range(i + 1, len(b)):
-            if abs(L.pnx_det_iou_bev_host(b[i].ctypes.data, b[j].ctypes.data) - thr) < margin:
-                return False
-    return True
+    b = boxes7.numpy()
+    i, j = np.triu_indices(len(b), 1)
+    return not (np.abs(ops.det_iou_bev_host(b[i], b[j]).astype(np.float64) - thr) < margin).any()
 
 
 def run_and_compare(pd, C, t, cfg, pre_max, post_max, label_offset=0):

@@ -72,7 +72,7 @@ def test_voxelize_waymo_shape_and_tiny():
 
 def frames_supported(batch, cfg):
     g = ops.grid_size_xy(cfg["voxel_size"], cfg["pc_range"])
-    return bool(ops.lib().pnx_voxelize_frames_supported(batch, int(g[0]), int(g[1])))
+    return bool(ops.voxelize_frames_supported(batch, int(g[0]), int(g[1])))
 
 
 @pytest.mark.parametrize("n,batch,kind", [(30000, 1, "uniform"), (30001, 2, "lidar"), (1001, 3, "uniform"), (257, 1, "uniform"),

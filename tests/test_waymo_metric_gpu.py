@@ -11,7 +11,7 @@ import torch
 
 from oracle import waymo_fixtures
 from oracle import waymo_metric_oracle as O
-from pillarnext_b200 import _lib, evaluate_waymo as EW
+from pillarnext_b200 import evaluate_waymo as EW, ops
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -35,23 +35,16 @@ def test_count_kernel_equals_host_twin():
     c_h = EW.run_host(pk)[0]
     assert np.array_equal(c_d, c_h)
     assert c_d.sum() > 24 * 50000 and (c_d == 0).sum() > 0 and ((c_d >= 1) & (c_d <= 5)).sum() > 0
-    L = _lib.lib()
     for f, t in enumerate(list(gts)[:4]):                       # the point test of ground-truth sampling, summed
         g = gts[t]
-        b = np.ascontiguousarray(g["boxes"])
-        trig = np.ascontiguousarray(pk["count_trig"][f, :len(b)])
-        pts = np.ascontiguousarray(g["points"])
-        inside = np.zeros((len(pts), len(b)), np.uint8)
-        _lib.check(L.pnx_points_in_boxes_host(pts.ctypes.data, len(pts), pts.shape[1], b.ctypes.data, trig.ctypes.data,
-                                              len(b), inside.ctypes.data))
-        assert np.array_equal(inside.sum(0), c_d[f, :len(b)])
+        inside = ops.points_in_boxes_host(g["points"], g["boxes"], pk["count_trig"][f, :len(g["boxes"])])
+        assert np.array_equal(inside.sum(0), c_d[f, :len(g["boxes"])])
 
 
 def test_pair_skip_never_hides_an_overlap():
     """Touching, barely overlapping and margin-distance (within in_box2d's 1e-2) rotated pairs, one pair per frame: the
     match's IoU (device and host) must equal the full routine's wherever it is 0, and bit for bit on the device/host."""
     rng = np.random.default_rng(5)
-    L = _lib.lib()
     n = 4000
     a = np.zeros((n, 9), np.float32)
     a[:, :2] = rng.uniform(-70, 70, (n, 2))
@@ -69,8 +62,7 @@ def test_pair_skip_never_hides_an_overlap():
         c, s = np.cos(box[:, 8]), np.sin(box[:, 8])
         return 0.5 * (box[:, 3] * np.abs(dirs[:, 0] * c + dirs[:, 1] * s) + box[:, 4] * np.abs(-dirs[:, 0] * s + dirs[:, 1] * c))
     def full_iou(b):                                            # the full routine, host-compiled, detection first
-        b7, a7 = np.ascontiguousarray(b[:, [0, 1, 2, 3, 4, 5, 8]]), np.ascontiguousarray(a[:, [0, 1, 2, 3, 4, 5, 8]])
-        return np.array([L.pnx_aligned_iou3d_host(b7[i].ctypes.data, a7[i].ctypes.data) for i in range(n)], np.float32)
+        return ops.aligned_iou3d_host(b[:, [0, 1, 2, 3, 4, 5, 8]], a[:, [0, 1, 2, 3, 4, 5, 8]])
     lo, hi = np.zeros(n), support(a, u) + support(b, u) + 1.0
     for _ in range(40):                                         # bisect the touching distance along u
         mid = 0.5 * (lo + hi)

@@ -31,7 +31,7 @@ def _use_sms(monkeypatch, sms, cx, cy, taps, M):
     if sms is None:
         return
     monkeypatch.setattr(ops, "sm_count", lambda: sms)
-    splits = ops.lib().pnx_wgrad_splits(cx, cy, taps, M, ops.sm_count())
+    splits = ops.wgrad_splits(cx, cy, taps, M, ops.sm_count())
     if sms == 1:
         assert splits <= 2, "%d K splits with one SM" % splits
     else:
@@ -185,7 +185,7 @@ def test_wgrad_deterministic_partials_are_bitwise_reproducible():
     ref = run()
     prev = ops.set_deterministic(True)
     try:
-        assert ops.lib().pnx_wgrad_splits(cx, cy, 9, M, ops.sm_count()) > 1, "the case must exercise several K splits"
+        assert ops.wgrad_splits(cx, cy, 9, M, ops.sm_count()) > 1, "the case must exercise several K splits"
         a, b = run(), run()
         acc = torch.ones(9, cx, cy, device="cuda")          # accumulates into dW like the atomic path
         ops.wgrad(X, cx, Y, cy, M, 9, acc, dense=geo)

@@ -21,7 +21,7 @@ def test_wgrad_64_channel_x_matches_the_full_block(cy, taps, shuffle):
         M, ry, geo = B * H * W, B * H * W, (H, W, H, W, 3, 1, 1, 1) if taps == 9 else None
     X = torch.randn(M, 128, device="cuda").bfloat16()
     Y = torch.randn(ry, cy, device="cuda").bfloat16()
-    assert ops.lib().pnx_wgrad_splits(64, cy, taps, M, ops.sm_count()) == ops.lib().pnx_wgrad_splits(128, cy, taps, M, ops.sm_count())
+    assert ops.wgrad_splits(64, cy, taps, M, ops.sm_count()) == ops.wgrad_splits(128, cy, taps, M, ops.sm_count())
     full = torch.zeros(taps, 128, cy, device="cuda")
     ops.wgrad(X, 128, Y, cy, M, taps, full, dense=geo, shuffle=shuffle)
     x64 = X[:, :64].contiguous()

@@ -58,7 +58,7 @@ def _split_cases(cases):
 def test_window_wgrad_matches_fp64(B, H, W, cx, cy, sms, monkeypatch):
     if sms is not None:
         monkeypatch.setattr(ops, "sm_count", lambda: sms)
-        splits, M = ops.lib().pnx_wgrad_splits(cx, cy, 9, B * H * W, sms), B * H * W
+        splits, M = ops.wgrad_splits(cx, cy, 9, B * H * W, sms), B * H * W
         assert (splits <= 2) if sms == 1 else (splits * 1024 >= M), "%d K splits of %d rows with %d SMs" % (splits, M, sms)
     torch.manual_seed(B * 1000 + H + W + cx + cy)
     X = torch.randn(B * H * W, cx, device="cuda").bfloat16()
@@ -109,7 +109,7 @@ def test_window_and_gather_paths_agree_bit_for_bit(B, H, W, cx, cy, deterministi
     finally:
         ops.set_deterministic(prev)
     if deterministic:
-        assert ops.lib().pnx_wgrad_splits(cx, cy, 9, M, ops.sm_count()) > 1
+        assert ops.wgrad_splits(cx, cy, 9, M, ops.sm_count()) > 1
     _close(window, _ref(X, Y, B, H, W))
     assert torch.equal(window, gather)
 

@@ -26,16 +26,13 @@ for (M, C, n) in [(677376, 384, 6), (169344, 256, 14), (677376, 64, 6), (140000,
     mean = torch.randn(C, device=dev) * 0.1; invstd = torch.rand(C, device=dev) + 0.5
     gamma = torch.ones(C, device=dev)
     red = torch.zeros(2 * C, dtype=torch.float64, device=dev)
-    L = ops.lib()
     t_apply = timeit(lambda: ops.bn_apply(x, M, C, sc, sh, y, relu=True))
     def reduce_only():
-        ops.check(L.pnx_bn_bwd_reduce(ops.ptr(dy), C, None, 8, ops.ptr(x), C, M, C, ops.ptr(mean), ops.ptr(invstd), 1,
-                                      ops.ptr(sc), ops.ptr(sh), ops.ptr(red), ops.stream()))
-    def apply_only():
-        ops.bn_bwd(dy, None, x, M, C, mean, invstd, gamma, M, True, dx, affine=(sc, sh), red=red)
+        ops.bn_bwd_reduce(dy, None, x, M, C, mean, invstd, True, (sc, sh), red=red)
+    def apply_only():   # the apply after a reduce fused into the GEMM epilogue: dy is the gated g, no mask
+        ops.bn_bwd_apply(dy, None, x, M, C, mean, invstd, gamma, red, M, False, (sc, sh), dx)
     def apply_mask():   # the un-fused apply: recomputed ReLU mask
-        ops.check(L.pnx_bn_bwd_apply(ops.ptr(dy), C, None, 8, ops.ptr(x), C, M, C, ops.ptr(mean), ops.ptr(invstd), ops.ptr(gamma),
-                                     ops.ptr(red), float(M), None, 1, ops.ptr(sc), ops.ptr(sh), ops.ptr(dx), C, None, 8, 0, ops.stream()))
+        ops.bn_bwd_apply(dy, None, x, M, C, mean, invstd, gamma, red, M, True, (sc, sh), dx)
     t_red, t_app, t_appm = timeit(reduce_only), timeit(apply_only), timeit(apply_mask)
     b = M * C * 2
     tot["apply"] += n * t_apply; tot["reduce"] += n * t_red; tot["bwd_apply"] += n * t_appm

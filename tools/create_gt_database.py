@@ -25,15 +25,9 @@ if ROOT not in sys.path:
 def points_in_rbbox(points, boxes):
     """[n, >= 3] fp32 points x [m, 9] fp32 boxes -> [n, m] bool (box_np_ops.points_in_rbbox, libm cosf / sinf)."""
     from det3d.datasets.pipelines.sample_ops import libm_trig
-    from pillarnext_b200 import _lib
-    points = np.ascontiguousarray(points, dtype=np.float32)
-    boxes = np.ascontiguousarray(boxes, dtype=np.float32).reshape(-1, 9)
-    trig = np.ascontiguousarray(libm_trig(boxes[:, -1]))
-    out = np.zeros((len(points), len(boxes)), dtype=np.uint8)
-    rc = _lib.lib().pnx_points_in_boxes_host(points.ctypes.data, len(points), points.shape[1], boxes.ctypes.data,
-                                              trig.ctypes.data, len(boxes), out.ctypes.data)
-    _lib.check(rc)
-    return out.astype(bool)
+    from pillarnext_b200 import ops
+    boxes = np.asarray(boxes, dtype=np.float32).reshape(-1, 9)
+    return ops.points_in_boxes_host(np.asarray(points, dtype=np.float32), boxes, libm_trig(boxes[:, -1]))
 
 
 def create_groundtruth_database(dataset, data_path, used_classes=None, db_path=None, dbinfo_path=None,
