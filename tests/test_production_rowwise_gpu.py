@@ -76,16 +76,19 @@ def arg_map(name):
 
 GEMM_REPLAYED = {"pnx_igemm", "pnx_conv3x3_win", "pnx_wgrad"}       # tests/test_production_gemms_gpu.py
 EXCLUDED = {
-    **dict.fromkeys(("pnx_voxelize", "pnx_voxelize_frames", "pnx_voxelize_frames_scratch", "pnx_voxelize_frames_supported",
-                     "pnx_voxelize_bitmap_words", "pnx_bucketize", "pnx_scan_u32", "pnx_scan_blocks", "pnx_blockcnt_size"),
-                    "voxelizer: edge cases and oracle parity in tests/test_voxelize_gpu.py"),
-    **dict.fromkeys(("pnx_sites_out_dim", "pnx_sites_dilate", "pnx_sites_inblock", "pnx_sites_coords", "pnx_nbr_table",
-                     "pnx_scatter_dense"), "sparse rulebook and densify: tests/test_rulebook_gpu.py"),
+    **dict.fromkeys(("pnx_voxelize", "pnx_voxelize_frames", "pnx_bucketize"),
+                    "voxelizer at the bench's shapes: tests/test_production_frontend_gpu.py"),
+    **dict.fromkeys(("pnx_sites_dilate", "pnx_scan_blocks", "pnx_sites_coords", "pnx_nbr_table", "pnx_scatter_dense"),
+                    "sparse rulebook and densify of the recorded pyramids: tests/test_production_frontend_gpu.py"),
     **dict.fromkeys(("pnx_pfn_mean", "pnx_pfn_lin0", "pnx_pfn_max0", "pnx_pfn_lin1", "pnx_pfn_max1", "pnx_pfn_backward"),
-                    "PillarFeatureNet: tests/test_voxelize_gpu.py and the fp64 edge cases of tests/test_sync_batchnorm_gpu.py"),
-    "pnx_pack_weights": "weight packing: tests/test_pack_gpu.py",
-    "pnx_assign_labels": "label assignment: tests/test_assign_gpu.py",
-    "pnx_aligned_iou3d": "IoU target of the Waymo `iou` head loss: tests/test_iou_loss_gpu.py",
+                    "PillarFeatureNet against float64 at the bench's shapes: tests/test_production_frontend_gpu.py"),
+    "pnx_pack_weights": "weight repack after AdamW: tests/test_production_frontend_gpu.py",
+    "pnx_assign_labels": "label assignment at the e2e shapes: tests/test_production_frontend_gpu.py",
+    "pnx_aligned_iou3d": "IoU target of the Waymo `iou` head loss: tests/test_production_frontend_gpu.py",
+    "pnx_scan_u32": "called inside pnx_bucketize (tests/test_production_frontend_gpu.py); launches nothing of its own here",
+    **dict.fromkeys(("pnx_voxelize_frames_scratch", "pnx_voxelize_frames_supported", "pnx_voxelize_bitmap_words",
+                     "pnx_blockcnt_size", "pnx_sites_out_dim"), "host-side size / geometry query; launches nothing"),
+    "pnx_sites_inblock": "not called by the step (the voxelizer writes level 0's inblk): tests/test_rulebook_gpu.py",
     "pnx_wgrad_splits": "host-side query of the weight-gradient split count; launches nothing",
     "pnx_set_deterministic": "mode switch; launches nothing",
     "pnx_split_get_pieces": "mode query of the split precision path; launches nothing",
