@@ -437,6 +437,31 @@ int pnx_gt_sample_host(const float* points, int n, const float* boxes, const int
 int pnx_points_in_boxes_host(const float* points, int n, int stride, const float* boxes, const float* trig, int m,
                              unsigned char* inside);
 
+/* ---------------------------------------------------------------- multi-sweep accumulation
+ * pnx_accumulate_sweeps: the reference's NuScenesDataset.load_pointcloud (read_sweep + remove_close) and
+ * WaymoDataset.load_pointcloud for a collated batch: past sweeps taken into the key frame and merged behind it.
+ *   points [n, 6] (batch_idx, x, y, z, intensity, time): the key frames, frame f owning rows point_off[f] ..
+ *   point_off[f + 1] - 1 (point_off [B + 1], from 0 to n);
+ *   sweep_points [S, 5] (x, y, z, intensity, time) in each sweep's own frame, time already the reference's fp32 value;
+ *   sweep (f, k) owns rows sweep_off[f K + k] .. sweep_off[f K + k + 1] - 1 (sweep_off [B K + 1], from 0 to S; a missing
+ *   or dropped sweep is an empty segment); transforms [B, K, 4, 4] fp64 row-major, sweep -> key frame (nuScenes
+ *   transform_matrix, Waymo inv(pose) @ sweep_pose); a matrix whose [3][3] entry is NaN marks "no transform" (the xyz is
+ *   copied); min_distance: sweep points with |x| < d and |y| < d after the transform are dropped (nuScenes 1.0; 0 = off).
+ * Outputs (new memory):
+ *   points_out [n + S, 6]: per frame in frame order, its key-frame rows unchanged, then sweep 1, 2, ... (batch index f,
+ *     transformed xyz, intensity, time), each in input order; rows [*count, n + S) get batch index B and zeros.
+ *   count [1]: valid rows of points_out.
+ * Arithmetic: csrc/sweeps.cu.  Three launches on `stream` (two when min_distance = 0), no host sync, no allocation:
+ * `workspace` holds pnx_accumulate_sweeps_workspace(S, B) bytes of device memory (no initialisation needed).  The host
+ * twin takes HOST memory and needs no workspace. */
+long long pnx_accumulate_sweeps_workspace(int S, int B);
+int pnx_accumulate_sweeps(const float* points, int n, const int* point_off, int B, const float* sweep_points, int S,
+                          const int* sweep_off, int K, const double* transforms, float min_distance, float* points_out,
+                          int* count, void* workspace, cudaStream_t stream);
+int pnx_accumulate_sweeps_host(const float* points, int n, const int* point_off, int B, const float* sweep_points, int S,
+                               const int* sweep_off, int K, const double* transforms, float min_distance,
+                               float* points_out, int* count);
+
 /* ---------------------------------------------------------------- Waymo-style evaluation (pillarnext_b200/evaluate_waymo.py)
  * pnx_eval_count_points: counts [B, M] int32 = number of points inside each ground-truth box, with the reference's
  * points_in_boxes_jit test (the one pnx_gt_sample uses).  points [n, stride >= 4] with (batch_idx, x, y, z) in columns

@@ -96,6 +96,10 @@ _SIGS = {
     "pnx_gt_sample": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P, P, P],
     "pnx_gt_sample_host": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P],
     "pnx_points_in_boxes_host": [P, I, I, P, P, I, P],
+    # multi-sweep accumulation: past sweeps into the key frame, close-point removal, merge
+    "pnx_accumulate_sweeps_workspace": [I, I],
+    "pnx_accumulate_sweeps": [P, I, P, I, P, I, P, I, P, F, P, P, P, P],
+    "pnx_accumulate_sweeps_host": [P, I, P, I, P, I, P, I, P, F, P, P],
     # Waymo-style evaluation: point counts per ground-truth box and the greedy score-ordered match
     "pnx_eval_count_points": [P, L, I, P, P, P, I, I, P, P],
     "pnx_eval_count_points_host": [P, L, I, P, P, P, I, I, P],
@@ -107,6 +111,7 @@ _SIGS = {
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,
+            "pnx_accumulate_sweeps_workspace": ctypes.c_longlong,
             "pnx_det_iou_bev_host": ctypes.c_float, "pnx_aligned_iou3d_host": ctypes.c_float}
 
 

@@ -741,7 +741,24 @@ class SingleStageDetector(nn.Module):
         out["points"], out["gt_boxes_raw"], out["gt_classes"] = points, boxes, classes
         return out
 
+    SWEEP_KEYS = ("point_offsets", "sweep_points", "sweep_offsets", "sweep_transforms", "sweep_min_distance")
+
+    def accumulate_sweeps(self, example):
+        """Multi-sweep accumulation on the GPU: the past sweeps scenes.collate packed (sweep_* keys) are taken into their
+        key frames and merged behind them by ops.accumulate_sweeps -- what the reference's data-loader workers do in numpy
+        when they load a frame (nusc.py / waymo.py load_pointcloud), before the sampler and the augmentation.  The rows
+        past the valid count carry batch index B, which every later stage drops or passes on.  Returns the example
+        without the sweep keys."""
+        e = example
+        points, _ = ops.accumulate_sweeps(e["points"], e["point_offsets"], e["sweep_points"], e["sweep_offsets"],
+                                          e["sweep_transforms"], e["sweep_min_distance"])
+        out = {k: v for k, v in example.items() if k not in self.SWEEP_KEYS}
+        out["points"] = points
+        return out
+
     def training_step(self, example):
+        if "sweep_points" in example:
+            example = self.accumulate_sweeps(example)
         if "gts_boxes" in example:
             example = self.gt_sample(example)
         if "aug" in example:
@@ -764,7 +781,10 @@ class SingleStageDetector(nn.Module):
     def validation_step(self, example):
         """Eval forward + predict -> {token: detections on the host}.  With `post_processing.double_flip` set, every
         frame runs four times (as is, mirrored in y, in x, in both: ops.flip4_points on the device, frames 4b + k) and
-        predict merges the four head outputs of each frame before decoding; the result is still one entry per token."""
+        predict merges the four head outputs of each frame before decoding; the result is still one entry per token.
+        An example with past sweeps (sweep_* keys) has them accumulated first."""
+        if "sweep_points" in example:
+            example = self.accumulate_sweeps(example)
         if self.post_processing is not None and _cfg_get(self.post_processing, "double_flip", False):
             flipped = dict(example)
             flipped["points"] = ops.flip4_points(example["points"].float())

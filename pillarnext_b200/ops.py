@@ -1041,6 +1041,47 @@ def gt_sample_host(points, gt_boxes, gt_classes, gt_trig, cand_boxes, cand_class
     return pts_out, box_out, cls_out, accepted, int(count[0])
 
 
+def _sweeps_operands(points, point_offsets, sweep_points, sweep_offsets, transforms, host=False):
+    B, K = transforms.shape[:2] if transforms.ndim == 4 else (len(point_offsets) - 1, 0)
+    f32, i32 = torch.float32, torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (points, f32, (len(points), 6), "points (batch_idx, x, y, z, intensity, time)"),
+        (point_offsets, i32, (B + 1,), "point_offsets"), (sweep_points, f32, (len(sweep_points), 5), "sweep_points"),
+        (sweep_offsets, i32, (B * K + 1,), "sweep_offsets"), (transforms, torch.float64, (B, K, 4, 4), "transforms"))]
+
+
+def accumulate_sweeps(points, point_offsets, sweep_points, sweep_offsets, transforms, min_distance):
+    """Multi-sweep accumulation on the GPU (pnx_accumulate_sweeps, include/pnx.h): the reference's nuScenes / Waymo
+    load_pointcloud for the sweeps scenes.collate packed (all CUDA tensors): key-frame points [n, 6] fp32 with frame f
+    owning rows point_offsets[f] .. point_offsets[f + 1] - 1 ([B + 1] int32), sweep_points [S, 5] fp32 in each sweep's
+    frame, sweep_offsets [B K + 1] int32 (sweep (f, k) = segment f K + k), transforms [B, K, 4, 4] fp64 (NaN [3][3] = no
+    transform), min_distance (1.0 nuScenes, 0 = off) -> (points [n + S, 6], count [1] int32 cuda).  Per frame, its key
+    points then its sweeps in order; the rows past `count` have batch index B, which the voxelizers drop; the host does
+    not wait for the count.  The inputs are left untouched."""
+    p, po, sp, so, tr = _sweeps_operands(points, point_offsets, sweep_points, sweep_offsets, transforms)
+    n, S, (B, K) = len(p), len(sp), tr.shape[:2]
+    dev = p.device
+    pts_out = torch.empty((n + S, 6), dtype=torch.float32, device=dev)
+    count = torch.empty(1, dtype=torch.int32, device=dev)
+    ws = torch.empty(max(4, lib().pnx_accumulate_sweeps_workspace(S, B)), dtype=torch.uint8, device=dev)
+    _count(3 if min_distance > 0 else 2)
+    check(lib().pnx_accumulate_sweeps(ptr(p), n, ptr(po), B, ptr(sp), S, ptr(so), K, ptr(tr), float(min_distance),
+                                      ptr(pts_out), ptr(count), ptr(ws), stream()))
+    return pts_out, count
+
+
+def accumulate_sweeps_host(points, point_offsets, sweep_points, sweep_offsets, transforms, min_distance):
+    """Host twin of accumulate_sweeps (pnx_accumulate_sweeps_host): the same operands as numpy arrays -> (points, count),
+    points a new array and count an int."""
+    p, po, sp, so, tr = _sweeps_operands(points, point_offsets, sweep_points, sweep_offsets, transforms, host=True)
+    n, S, (B, K) = len(p), len(sp), tr.shape[:2]
+    pts_out = np.full((n + S, 6), np.nan, np.float32)           # every row is written: a NaN left over is a twin's bug
+    count = np.zeros(1, np.int32)
+    check(lib().pnx_accumulate_sweeps_host(_hp(p), n, _hp(po), B, _hp(sp), S, _hp(so), K, _hp(tr), float(min_distance),
+                                           _hp(pts_out), _hp(count)))
+    return pts_out, int(count[0])
+
+
 def _row_shape(t, min_cols, what):
     """Shape (n, c) of a [n, >= min_cols] operand; raises otherwise."""
     shape = tuple(getattr(t, "shape", ()))

@@ -97,6 +97,55 @@ def make_scene(seed, cfg, n_points=6000, n_boxes=12):
     return pts[g.permutation(len(pts))], boxes.astype(np.float32), names
 
 
+def ego_pose(seed, lag, ego_speed):
+    """4x4 fp64 transform from the sensor frame `lag` seconds before key frame `seed` to the key frame: the ego drives a
+    seeded planar arc (heading, speed up to ego_speed m/s, yaw rate up to 0.3 rad/s) and sits at the origin at lag 0."""
+    g = np.random.default_rng([290000, seed])
+    heading, speed, rate = g.uniform(-np.pi, np.pi), ego_speed * g.uniform(0.5, 1.0), g.uniform(-0.3, 0.3)
+    th = -rate * lag
+    c, s = np.cos(th), np.sin(th)
+    T = np.eye(4)
+    T[:2, :2] = [[c, -s], [s, c]]
+    T[:2, 3] = -speed * lag * np.array([np.cos(heading + th / 2), np.sin(heading + th / 2)])
+    return T
+
+
+def make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=0.05, ego_speed=5.0):
+    """Past sweep k >= 1 of key frame `seed` (boxes: its gt_boxes [M, 9]), scanned k * sweep_interval seconds earlier:
+    each box at centre - v * lag (v = its vx, vy label; barriers and cones do not move), seen from that sweep's sensor
+    pose (ego_pose).  Returns (points [N, 5] fp32 in the sweep's sensor frame with time = float32(lag), like a .bin
+    file; transform_matrix [4, 4] fp64 sweep -> key frame; box_index [N] int, the box a point was sampled on or -1).
+    Its own seeded streams: the key frame stays exactly make_scene(seed)."""
+    lag = k * sweep_interval
+    T = ego_pose(seed, lag, ego_speed)
+    g = np.random.default_rng([390000, seed, k])
+    b = boxes.astype(np.float64).copy()
+    b[:, :2] -= b[:, 6:8] * lag                                     # key-frame position at the sweep's time
+    R, t = T[:2, :2], T[:2, 3]
+    b[:, :2] = (b[:, :2] - t) @ R                                   # into the sweep's sensor frame: R^T (c - t)
+    b[:, 8] -= np.arctan2(T[1, 0], T[0, 0])
+    ground = synth.make_frame(1000003 * (k + 1) + seed, int(n_points * 0.7), cfg, kind="lidar")[:, :3].astype(np.float64)
+    keep = np.ones(len(ground), dtype=bool)
+    for bb in b:
+        c, s = np.cos(-bb[8]), np.sin(-bb[8])
+        lx = (ground[:, 0] - bb[0]) * c - (ground[:, 1] - bb[1]) * s
+        ly = (ground[:, 0] - bb[0]) * s + (ground[:, 1] - bb[1]) * c
+        keep &= ~((np.abs(lx) < bb[3] / 2) & (np.abs(ly) < bb[4] / 2))
+    parts, owner = [ground[keep]], [np.full(int(keep.sum()), -1)]
+    budget = n_points - int(keep.sum())
+    if len(b):
+        w = np.array([(bb[3] * bb[5] + bb[4] * bb[5]) / max(np.hypot(bb[0], bb[1]), 3.0) ** 1.2 for bb in b])
+        per = np.clip((budget * w / w.sum()).astype(int), 25, 600)
+        for j, (bb, m) in enumerate(zip(b, per)):
+            parts.append(_box_surface_points(g, bb[[0, 1, 2, 3, 4, 5, 8]], int(m)))
+            owner.append(np.full(len(parts[-1]), j))
+    xyz, owner = np.concatenate(parts, 0), np.concatenate(owner, 0)
+    inten = g.uniform(0, cfg["intensity_max"], (len(xyz), 1))
+    pts = np.concatenate([xyz, inten, np.full((len(xyz), 1), np.float32(lag))], 1).astype(np.float32)
+    order = g.permutation(len(pts))
+    return pts[order], T, owner[order]
+
+
 class SyntheticSceneDataset(torch.utils.data.Dataset):
     """Frames are generated on the fly from (seed0 + index): an unbounded, reproducible stream; train and held-out
     splits are disjoint seed ranges.
@@ -109,12 +158,26 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     (sample_ops.DataBaseSamplerV2.sample_all; none drawn = zero candidates) and numpy's (cos, sin) of the scene boxes'
     yaws.  root_path is where the sampler node's `${data.train_dataset.root_path}` points (the gt database).
 
+    nsweeps, drop_frames: past sweeps accumulated into every frame, as the reference's nuScenes (nsweeps 10) and Waymo
+    (nsweeps 3, drop_frames 0.5 in training) datasets do.  With nsweeps > 1 each frame gets a `sweeps` record of its
+    nsweeps - 1 past sweeps (make_sweep: the ego and the objects move, sweep_interval seconds apart, the ego at up to
+    ego_speed m/s); each is dropped with probability drop_frames by one np.random.uniform() draw per sweep, in sweep
+    order and before the sampler and the augmentation draw anything (waymo.py:55-57, base.py:69-99).  The detector
+    takes the sweeps into the key frame on the GPU (ops.accumulate_sweeps), dropping the sweep points within
+    min_distance of the sensor in x and y (nuScenes' remove_close; 0 = off).  nsweeps = 1 frames are unchanged.
+
     metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map), "waymo" (evaluate_waymo.waymo_metrics,
     AP / APH at LEVEL_1 and LEVEL_2) or "nds" (evaluate_nuscenes.nuscenes_metrics, the nuScenes detection score with
     its true-positive errors).  For "waymo" and "nds" ground_truth() also hands over each frame's points."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
-                 augmentation=None, sampler=None, root_path=None, metric="nuscenes", **_):
+                 augmentation=None, sampler=None, root_path=None, metric="nuscenes", nsweeps=1, drop_frames=0.0,
+                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, **_):
+        if int(nsweeps) < 1 or not 0.0 <= drop_frames <= 1.0 or min_distance < 0:
+            raise ValueError("nsweeps must be >= 1, drop_frames in [0, 1] and min_distance >= 0, got %r, %r, %r"
+                             % (nsweeps, drop_frames, min_distance))
+        self.nsweeps, self.drop_frames = int(nsweeps), float(drop_frames)
+        self.sweep_interval, self.ego_speed, self.min_distance = float(sweep_interval), float(ego_speed), float(min_distance)
         self.cfg, self.n_frames, self.seed0, self.n_points, self.n_boxes = cfg, int(n_frames), int(seed0), int(n_points), int(n_boxes)
         self.test_mode = test_mode
         if metric not in ("nuscenes", "waymo", "nds"):
@@ -138,12 +201,28 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
         cls = np.array([self.class_names.index(n) for n in names], dtype=np.int32)
         res = {"points": pts, "gt_boxes_raw": boxes, "gt_classes": cls, "token": "scene_%d" % (self.seed0 + i)}
+        if self.nsweeps > 1:
+            res["sweeps"] = self._sweeps(self.seed0 + i, boxes)
         if self.sampler is not None:
             res["gts"] = self._candidates(boxes, names)
         if self.augmentations is not None:
             for aug in self.augmentations.values():
                 res = aug(res)
         return res
+
+    def _sweeps(self, seed, boxes):
+        kept = [not (self.drop_frames > 0 and np.random.uniform() < self.drop_frames) for _ in range(self.nsweeps - 1)]
+        pts, counts, tms = [], [], []
+        for k, keep in enumerate(kept, 1):
+            if keep:
+                p, T, _ = make_sweep(seed, k, self.cfg, boxes, self.n_points, self.sweep_interval, self.ego_speed)
+            else:
+                p, T = np.zeros((0, 5), np.float32), np.full((4, 4), np.nan)
+            pts.append(p)
+            counts.append(len(p))
+            tms.append(T)
+        return {"points": np.concatenate(pts, 0), "counts": np.array(counts, np.int64), "transforms": np.stack(tms),
+                "min_distance": self.min_distance}
 
     def _candidates(self, boxes, names):
         from det3d.datasets.pipelines.sample_ops import numpy_trig
@@ -190,7 +269,12 @@ def collate(batch_list):
       gts_boxes [B, S, 9] fp32, gts_classes [B, S] int32 (-1 = padding), gts_trig [B, S, 4] fp32   the candidates
       gts_points [P, 5] fp32, gts_offsets [B S + 1] int32    their stored points; candidate (b, s) owns rows
                                                              gts_offsets[b S + s] .. gts_offsets[b S + s + 1] - 1
-      gt_trig [B, M, 2] fp32                                 numpy's (cos, sin) of the scene boxes' yaws"""
+      gt_trig [B, M, 2] fp32                                 numpy's (cos, sin) of the scene boxes' yaws
+    Frames with past sweeps (`sweeps`) add, with K the most sweeps of any frame (a dropped sweep is an empty slot):
+      point_offsets [B + 1] int32              frame f's key-frame points are rows point_offsets[f] .. [f + 1] - 1
+      sweep_points [S, 5] fp32, sweep_offsets [B K + 1] int32   sweep (f, k) owns rows sweep_offsets[f K + k] .. - 1
+      sweep_transforms [B, K, 4, 4] fp64       sweep -> key frame (NaN = no transform)
+      sweep_min_distance float                 the close-point radius of ops.accumulate_sweeps"""
     pts = [np.pad(b["points"], ((0, 0), (1, 0)), mode="constant", constant_values=i) for i, b in enumerate(batch_list)]
     m = max(1, max(len(b["gt_classes"]) for b in batch_list))
     boxes = np.zeros((len(batch_list), m, 9), dtype=np.float32)
@@ -236,4 +320,26 @@ def collate(batch_list):
         out.update(gts_boxes=torch.tensor(cb), gts_classes=torch.tensor(cc), gts_trig=torch.tensor(ct),
                    gts_points=torch.tensor(np.concatenate(pts, 0).astype(np.float32).reshape(-1, 5)),
                    gts_offsets=torch.tensor(off.astype(np.int32)), gt_trig=torch.tensor(st))
+    if any("sweeps" in b for b in batch_list):
+        if not all("sweeps" in b for b in batch_list):
+            raise ValueError("either every frame of a batch carries past sweeps or none does")
+        md = {b["sweeps"]["min_distance"] for b in batch_list}
+        if len(md) != 1:
+            raise ValueError("the frames of a batch must share one min_distance, got %s" % sorted(md))
+        B = len(batch_list)
+        K = max(1, max(len(b["sweeps"]["counts"]) for b in batch_list))
+        counts = np.zeros((B, K), np.int64)
+        tms = np.full((B, K, 4, 4), np.nan)
+        for i, b in enumerate(batch_list):
+            sw = b["sweeps"]
+            counts[i, :len(sw["counts"])], tms[i, :len(sw["counts"])] = sw["counts"], sw["transforms"]
+        off = np.concatenate([[0], np.cumsum(counts.reshape(-1))])
+        if off[-1] + len(out["points"]) >= 2 ** 31 - 1:
+            raise ValueError("too many points in one batch for int32 offsets")
+        key = np.concatenate([[0], np.cumsum([len(b["points"]) for b in batch_list])])
+        out.update(point_offsets=torch.tensor(key.astype(np.int32)),
+                   sweep_points=torch.tensor(np.concatenate([b["sweeps"]["points"] for b in batch_list], 0)
+                                             .astype(np.float32).reshape(-1, 5)),
+                   sweep_offsets=torch.tensor(off.astype(np.int32)), sweep_transforms=torch.tensor(tms),
+                   sweep_min_distance=float(md.pop()))
     return out
