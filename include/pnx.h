@@ -424,7 +424,8 @@ int pnx_global_aug_host(const float* points, int n, const float* boxes, int B, i
  * pnx_gt_sample_workspace(n, B, S) bytes of device memory (no initialisation needed).  B <= 512.  The host twin takes
  * HOST memory and needs no workspace.  pnx_points_in_boxes_host is the point test alone (box_np_ops.points_in_rbbox):
  * inside [n, m] bytes for points with x, y, z at the start of `stride`-float rows, 9-column boxes, and trig [m, 2] =
- * (cosf, sinf) of each yaw. */
+ * (cosf, sinf) of each yaw.  pnx_points_in_boxes is its device twin (csrc/det_eval.cu, equal to it to the bit): the same
+ * operands in device memory, one launch on `stream`, no host sync, no workspace. */
 long long pnx_gt_sample_workspace(int n, int B, int S);
 int pnx_gt_sample(const float* points, int n, const float* boxes, const int* classes, const float* box_trig, int B, int M,
                   const float* cand_boxes, const int* cand_classes, const float* cand_trig, int S, const float* cand_points,
@@ -436,6 +437,8 @@ int pnx_gt_sample_host(const float* points, int n, const float* boxes, const int
                        int* classes_out, int* accepted, int* count);
 int pnx_points_in_boxes_host(const float* points, int n, int stride, const float* boxes, const float* trig, int m,
                              unsigned char* inside);
+int pnx_points_in_boxes(const float* points, int n, int stride, const float* boxes, const float* trig, int m,
+                        unsigned char* inside, cudaStream_t stream);
 
 /* ---------------------------------------------------------------- multi-sweep accumulation
  * pnx_accumulate_sweeps: the reference's NuScenesDataset.load_pointcloud (read_sweep + remove_close) and

@@ -96,6 +96,7 @@ _SIGS = {
     "pnx_gt_sample": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P, P, P],
     "pnx_gt_sample_host": [P, I, P, P, P, I, I, P, P, P, I, P, P, I, P, P, P, P, P],
     "pnx_points_in_boxes_host": [P, I, I, P, P, I, P],
+    "pnx_points_in_boxes": [P, I, I, P, P, I, P, P],
     # multi-sweep accumulation: past sweeps into the key frame, close-point removal, merge
     "pnx_accumulate_sweeps_workspace": [I, I],
     "pnx_accumulate_sweeps": [P, I, P, I, P, I, P, I, P, F, P, P, P, P],

@@ -4,6 +4,8 @@
 //                          points_in_boxes_jit test (box_geom.cuh point_in_box); integer atomics, so the counts are exact
 //                          and do not depend on the schedule.  The counts decide each box's difficulty level (Waymo) or
 //                          drop the boxes without points (nuScenes).
+//   pnx_points_in_boxes    the same test for every (point, box) pair of one frame: the [n, m] mask the gt-database tool
+//                          cuts objects with (the device twin of gt_sample.cu's pnx_points_in_boxes_host).
 //   pnx_eval_match         one warp per (frame, class) segment of detections, pre-sorted by the 64-bit key
 //                          (segment << 32 | descending score, as postproc.cu's keys): the greedy score-ordered match.
 //                          For each detection in order the lanes compute its IoUs against the segment's still unmatched
@@ -108,6 +110,20 @@ __global__ void __launch_bounds__(256) eval_count_kernel(const float* __restrict
   for (int j = 0; j < M; ++j) {
     const long long k = (long long)f * M + j;
     if (classes[k] >= 0 && point_in_box(x, y, z, boxes + k * 9, trig[2 * k], trig[2 * k + 1])) atomicAdd(&counts[k], 1);
+  }
+}
+
+// inside[i m + j] = point i inside box j: one thread per (point, box) pair, so consecutive threads write consecutive bytes
+__global__ void __launch_bounds__(256) points_in_boxes_kernel(const float* __restrict__ points, long long n, int stride,
+                                                              const float* __restrict__ boxes,
+                                                              const float* __restrict__ trig, int m,
+                                                              unsigned char* __restrict__ inside) {
+  const long long total = n * m;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long i = e / m;
+    const int j = (int)(e - i * m);
+    const float* p = points + i * stride;
+    inside[e] = point_in_box(p[0], p[1], p[2], boxes + (long long)j * 9, trig[2 * j], trig[2 * j + 1]);
   }
 }
 
@@ -269,6 +285,18 @@ extern "C" int pnx_eval_count_points(const float* points, long long n, int strid
   PNX_CUDA(cudaMemsetAsync(counts, 0, (size_t)B * M * sizeof(int), stream));
   if (n == 0) return PNX_OK;
   eval_count_kernel<<<pnx_cdiv(n, 256), 256, 0, stream>>>(points, n, stride, boxes, classes, trig, B, M, counts);
+  PNX_CHECK_LAUNCH();
+  return PNX_OK;
+}
+
+extern "C" int pnx_points_in_boxes(const float* points, int n, int stride, const float* boxes, const float* trig, int m,
+                                   unsigned char* inside, cudaStream_t stream) {
+  PNX_CHECK_ARG(n >= 0 && m >= 0 && stride >= 3, "n / m / stride");
+  PNX_CHECK_ARG((long long)n * m == 0 || (points && boxes && trig && inside), "pointers");
+  if ((long long)n * m == 0) return PNX_OK;
+  const long long blocks = ((long long)n * m + 255) / 256;
+  points_in_boxes_kernel<<<(int)(blocks < 65536 ? blocks : 65536), 256, 0, stream>>>(points, n, stride, boxes, trig, m,
+                                                                                     inside);
   PNX_CHECK_LAUNCH();
   return PNX_OK;
 }

@@ -7,8 +7,9 @@ scoring to the devkit (det3d/datasets/waymo/waymo.py:124 writes a .bin for it), 
     max(vol_a + vol_b - overlap, 1e-6), in fp32, detection first -- the per-pair arithmetic of the `iou` head target.
   * Thresholds per class: vehicle 0.7, pedestrian 0.5, cyclist 0.5; any other class takes its threshold from the
     `iou_thresholds` mapping (which may also override these).  A class with neither raises ValueError.
-  * Difficulty: the frame's points inside each ground-truth box are counted with the reference's points_in_boxes_jit
-    test (libm cosf / sinf of the yaw).  A box with 0 points is dropped from evaluation, a box with 1-5 points is
+  * Difficulty: a frame's "num_points" (the label's point count, as the devkit reads it) where it gives them;
+    otherwise the frame's points inside each ground-truth box, counted with the reference's points_in_boxes_jit test
+    (libm cosf / sinf of the yaw).  A box with 0 points is dropped from evaluation, a box with 1-5 points is
     LEVEL_2, every other box LEVEL_1.
   * Matching, once per (frame, class): the detections are visited in descending score order, ties by lower index; each
     takes the unmatched ground-truth box with the highest IoU >= threshold, ties by lower index, or stays unmatched.
@@ -80,6 +81,7 @@ def pack(gts, detections, class_names, iou_thresholds=None):
     gt_boxes = np.zeros((B, M, 9), np.float32)
     gt_boxes[:, :, 3:6] = 1.0
     gt_classes = np.full((B, M), -1, np.int32)
+    num_points = np.full((B, M), -1, np.int64)
     points = []
     for f, t in enumerate(tokens):
         g = gts[t]
@@ -88,7 +90,14 @@ def pack(gts, detections, class_names, iou_thresholds=None):
             raise ValueError("frame %s: %d boxes but %d names" % (t, len(b), len(g["names"])))
         gt_boxes[f, :len(b)] = b
         gt_classes[f, :len(b)] = [cls_of.get(n, -1) for n in g["names"]]
-        p = _arr(g["points"], np.float32)
+        if "num_points" in g:
+            n = _arr(g["num_points"]).reshape(-1).astype(np.int64)
+            if len(n) != len(b) or (n < 0).any():
+                raise ValueError("frame %s: %d boxes but num_points %s" % (t, len(b), n))
+            num_points[f, :len(b)] = n
+        elif "points" not in g:
+            raise ValueError("frame %s: ground truth needs num_points or points for the difficulty levels" % t)
+        p = _arr(g["points"], np.float32) if "num_points" not in g else np.zeros((0, 3), np.float32)
         q = np.empty((len(p), 4), np.float32)
         q[:, 0] = f
         q[:, 1:] = p[:, :3]
@@ -121,7 +130,8 @@ def pack(gts, detections, class_names, iou_thresholds=None):
     seg_count = np.bincount(det_seg, minlength=B * C).astype(np.int32)
     seg_start = (np.cumsum(seg_count) - seg_count).astype(np.int32)
     return dict(B=B, M=M, C=C, thresholds=thr, points=np.concatenate(points) if points else np.zeros((0, 4), np.float32),
-                gt_boxes=gt_boxes, gt_classes=gt_classes, count_trig=count_trig, gt_trig=gt_trig, det_boxes=det_boxes,
+                gt_boxes=gt_boxes, gt_classes=gt_classes, num_points=num_points, count_trig=count_trig, gt_trig=gt_trig,
+                det_boxes=det_boxes,
                 det_scores=det_scores, det_labels=det_seg % C, det_frames=det_seg // C,
                 det_trig=heading_trig(det_boxes[:, 8]), keys=keys, seg_start=seg_start, seg_count=seg_count)
 
@@ -196,10 +206,16 @@ def score(pk, counts, match, heading, class_names):
 
 def waymo_metrics(gts, detections, class_names, iou_thresholds=None):
     """gts: token -> {"boxes" [M, 7 or 9] (x, y, z, dx, dy, dz, [vx, vy,] yaw), "names" list[str], "points" [N, >= 3]
-    (x, y, z first)}; detections: token -> {"box3d_lidar" [K, 9], "scores" [K], "label_preds" [K]} (the reference's
-    validation_step output, single_stage.py:47-59; CPU or CUDA tensors, or arrays), labels indexing class_names.
+    (x, y, z first) or "num_points" [M] (each label's point count, as the devkit takes it)}; detections: token ->
+    {"box3d_lidar" [K, 9], "scores" [K], "label_preds" [K]} (the reference's validation_step output,
+    single_stage.py:47-59; CPU or CUDA tensors, or arrays), labels indexing class_names.
     Ground-truth boxes whose name is not in class_names are not evaluated.  Returns {"mAP_L1", "mAPH_L1", "mAP_L2",
     "mAPH_L2", "per_class": {name: {AP_L1, APH_L1, AP_L2, APH_L2, n_gt_L1, n_gt_L2}}}, AP values in percent."""
     pk = pack(gts, detections, class_names, iou_thresholds)
     counts, match, _, heading = run_device(pk)
-    return score(pk, counts, match, heading, class_names)
+    return score(pk, known_counts(pk, counts), match, heading, class_names)
+
+
+def known_counts(pk, counts):
+    """The point counts of the difficulty levels: a frame's "num_points" where it gives them, else the counted ones."""
+    return np.where(pk["num_points"] >= 0, pk["num_points"], counts)

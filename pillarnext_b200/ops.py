@@ -1090,14 +1090,31 @@ def _row_shape(t, min_cols, what):
     return shape
 
 
+def _points_in_boxes_operands(points, boxes, trig, host=False):
+    m = len(boxes)
+    return (_want(points, torch.float32, _row_shape(points, 3, "points"), "points", host),
+            _want(boxes, torch.float32, (m, 9), "boxes", host), _want(trig, torch.float32, (m, 2), "trig", host))
+
+
+def points_in_boxes(points, boxes, trig):
+    """The point test of gt_sample on the GPU (pnx_points_in_boxes, the reference's points_in_rbbox): points fp32
+    [n, >= 3] (x, y, z first), boxes [m, 9] fp32, trig [m, 2] fp32 = libm (cosf, sinf) of each yaw, all CUDA -> inside
+    [n, m] bool cuda, equal to points_in_boxes_host to the bit."""
+    points, boxes, trig = _points_in_boxes_operands(points, boxes, trig)
+    n, m = len(points), len(boxes)
+    inside = torch.empty((n, m), dtype=torch.uint8, device=points.device)
+    if n * m:
+        _count(1)
+    check(lib().pnx_points_in_boxes(ptr(points), n, points.shape[1], ptr(boxes), ptr(trig), m, ptr(inside), stream()))
+    return inside.view(torch.bool)
+
+
 def points_in_boxes_host(points, boxes, trig):
     """The point test of gt_sample on the host (pnx_points_in_boxes_host, the reference's points_in_rbbox): points numpy
     fp32 [n, >= 3] (x, y, z first), boxes [m, 9] fp32, trig [m, 2] fp32 = libm (cosf, sinf) of each yaw -> inside
     [n, m] bool."""
-    points = _want(points, torch.float32, _row_shape(points, 3, "points"), "points", host=True)
+    points, boxes, trig = _points_in_boxes_operands(points, boxes, trig, host=True)
     m = len(boxes)
-    boxes = _want(boxes, torch.float32, (m, 9), "boxes", host=True)
-    trig = _want(trig, torch.float32, (m, 2), "trig", host=True)
     inside = np.zeros((len(points), m), np.uint8)
     check(lib().pnx_points_in_boxes_host(_hp(points), len(points), points.shape[1], _hp(boxes), _hp(trig), m, _hp(inside)))
     return inside.astype(bool)

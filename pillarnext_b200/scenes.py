@@ -146,6 +146,26 @@ def make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=0.05, ego_speed=5.0
     return pts[order], T, owner[order]
 
 
+def sampling_record(sampler, boxes, names, class_names):
+    """The `gts` record of one frame: the candidates sampler.sample_all draws for the scene boxes [M, 9] fp32 named
+    `names` (none drawn = zero candidates), their classes as indices into class_names, and numpy's (cos, sin) of the
+    scene boxes' yaws."""
+    from det3d.datasets.pipelines.sample_ops import numpy_trig
+    rec = sampler.sample_all(boxes, np.array(names))
+    if rec is None:
+        rec = {"gt_names": np.zeros(0, dtype=str), "gt_boxes": np.zeros((0, 9), np.float32),
+               "points": np.zeros((0, 5), np.float32), "num_points": np.zeros(0, np.int64),
+               "trig": np.zeros((0, 4), np.float32)}
+    if rec["points"].shape[1] != 5:
+        raise ValueError("the sampler's point_dim must be 5 (x, y, z, intensity, time), got %d" % rec["points"].shape[1])
+    unknown = sorted(set(rec["gt_names"]) - set(class_names))
+    if unknown:
+        raise ValueError("sampled classes %s are not classes of this dataset" % unknown)
+    return {"boxes": rec["gt_boxes"], "classes": np.array([class_names.index(n) for n in rec["gt_names"]], np.int32),
+            "points": rec["points"], "num_points": rec["num_points"], "trig": rec["trig"],
+            "scene_trig": numpy_trig(boxes)}
+
+
 class SyntheticSceneDataset(torch.utils.data.Dataset):
     """Frames are generated on the fly from (seed0 + index): an unbounded, reproducible stream; train and held-out
     splits are disjoint seed ranges.
@@ -225,20 +245,7 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
                 "min_distance": self.min_distance}
 
     def _candidates(self, boxes, names):
-        from det3d.datasets.pipelines.sample_ops import numpy_trig
-        rec = self.sampler.sample_all(boxes, np.array(names))
-        if rec is None:
-            rec = {"gt_names": np.zeros(0, dtype=str), "gt_boxes": np.zeros((0, 9), np.float32),
-                   "points": np.zeros((0, 5), np.float32), "num_points": np.zeros(0, np.int64),
-                   "trig": np.zeros((0, 4), np.float32)}
-        if rec["points"].shape[1] != 5:
-            raise ValueError("the sampler's point_dim must be 5 (x, y, z, intensity, time), got %d" % rec["points"].shape[1])
-        unknown = sorted(set(rec["gt_names"]) - set(self.class_names))
-        if unknown:
-            raise ValueError("sampled classes %s are not classes of this dataset" % unknown)
-        return {"boxes": rec["gt_boxes"], "classes": np.array([self.class_names.index(n) for n in rec["gt_names"]], np.int32),
-                "points": rec["points"], "num_points": rec["num_points"], "trig": rec["trig"],
-                "scene_trig": numpy_trig(boxes)}
+        return sampling_record(self.sampler, boxes, names, self.class_names)
 
     def ground_truth(self):
         gts = {}
