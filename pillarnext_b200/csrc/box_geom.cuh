@@ -116,11 +116,16 @@ __host__ __device__ inline bool seg_intersection(const P2& p1, const P2& p0, con
   return true;
 }
 
+// The axis-aligned corners x1 = x - dx / 2, ... are rounded first and rotated about the centre as (x1 - x), ...: the
+// reference's form.  (x1 - x) is not -dx / 2 in fp32, so writing the offsets as +-dx / 2 directly moves corners by an
+// ulp of the centre and flips decisions near the threshold.
 template <class T>
 __host__ __device__ inline void box_corners(const float* box, const T& tr, P2* c5) {
   const float hx = box[3] / 2, hy = box[4] / 2;
+  const float x1 = box[0] - hx, y1 = box[1] - hy, x2 = box[0] + hx, y2 = box[1] + hy;
   const float ca = tr.cos_h(), sa = tr.sin_h();
-  const float px[4] = {-hx, hx, hx, -hx}, py[4] = {-hy, -hy, hy, hy};
+  const float px[4] = {x1 - box[0], x2 - box[0], x2 - box[0], x1 - box[0]};
+  const float py[4] = {y1 - box[1], y1 - box[1], y2 - box[1], y2 - box[1]};
   for (int k = 0; k < 4; ++k) {
     c5[k].x = px[k] * ca + py[k] * (-sa) + box[0];
     c5[k].y = px[k] * sa + py[k] * ca + box[1];

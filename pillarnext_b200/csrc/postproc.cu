@@ -18,9 +18,13 @@
 // Provenance note: the rotated-rectangle overlap routines (box_geom.cuh: cross3, rect_cross, in_box2d, seg_intersection,
 // det_box_overlap, det_iou_bev) deliberately follow the ARITHMETIC of the reference's own device code,
 // det3d/core/iou3d_nms/src/iou3d_nms_kernel.cu:39-235 (and its host twin iou3d_cpu.cpp), statement by statement -- same
-// operation order, same 1e-2 margin, same angular ordering of the polygon vertices: the keep / suppress decision of every
-// box pair must come out bit-identical to the reference's NMS, and any algebraically equivalent rewrite flips decisions for
-// IoUs near the threshold.  Everything around them (fused decode, 64-bit sort keys, batched per-(frame, class) mask, the
+// operation order (corners rounded as x - dx / 2 and rotated as (x1 - x)), same 1e-2 margin, same angular ordering of
+// the polygon vertices: any algebraically equivalent rewrite flips decisions for IoUs near the threshold.  Which builds
+// this matches: this file as compiled by build.py (nvcc -O3, fp32 contraction on) against the reference's nms_gpu
+// compiled for sm_90a with nvcc's defaults (contraction on; oracle/build_ref_nms.py): equal keep lists at the bench's
+// configurations and on segments built to sit on the threshold (tests/test_production_postproc_gpu.py); the host twin
+// (no FMA) against iou3d_cpu.cpp built by g++ without FMA: bit-identical IoUs (tests/test_predict_cpu.py).  A device
+// build with different contraction is not covered by either.  Everything around them (fused decode, 64-bit sort keys, batched per-(frame, class) mask, the
 // on-GPU sweep with up to 4 slots of 2048 candidates, `__host__ __device__` for the CPU parity leg) is this repository's.
 // Hot loop character: HBM-bound single pass (1) and a few hundred thousand polygon clips (2) -- no tensor-core work.
 #include <math.h>

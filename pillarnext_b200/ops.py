@@ -893,7 +893,7 @@ def det_postprocess(out, B, H, W, C, offs, osf, voxel_size, pc_range, score_thr,
                                   (L.pnx_det_keys, L.pnx_det_nms, L.pnx_det_gather))
     _count(1)
     check(keys_fn(*common, ptr(keys), ptr(seg_count), stream()))
-    order = torch.sort(keys)[1]
+    order = torch.sort(keys, stable=True)[1]        # tied scores: ascending pixel index, whatever sort torch picks
     seg_start = (torch.cumsum(seg_count, 0, dtype=torch.int32) - seg_count).contiguous()
     col_blocks = (pre_max + 63) // 64
     mask = torch.empty(nseg * pre_max * col_blocks, dtype=torch.int64, device=dev)

@@ -111,6 +111,18 @@ def test_host_compiled_decode_and_iou_match_oracle():
         assert abs(float(got[i // 2]) - float(P.iou_bev(bx[i], bx[i + 1]))) < 2e-6
 
 
+def test_host_compiled_iou_equals_reference_extension_bit_for_bit():
+    """The product's rotated IoU compiled for the host equals the reference's iou3d_cpu.cpp (golden) to the bit on every
+    pair: the same statements in the same order, down to the corners rounded as x - dx / 2 before the rotation."""
+    from pillarnext_b200 import ops
+    a, b = rand_boxes(24, 1).numpy(), rand_boxes(24, 2).numpy()
+    want = np.load(os.path.join(GOLDEN, "ref_live.npz"))["iou_bev"]
+    got = ops.det_iou_bev_host(np.repeat(a, 24, 0), np.tile(b, (24, 1))).reshape(24, 24)
+    assert (want > 0).sum() > 200
+    assert np.array_equal(got.view(np.int32), want.view(np.int32)), "%d of 576 pairs differ" % int(
+        (got.view(np.int32) != want.view(np.int32)).sum())
+
+
 def test_oracle_predict_matches_golden_reference_outputs():
     """Runs anywhere: tests/golden/ref_predict.npz holds the reference's own predict outputs (oracle/make_golden_predict.py)."""
     from oracle.make_golden_predict import SEEDS, SHAPE, TASKS
