@@ -9,7 +9,8 @@ transform inv(pose) @ sweep_pose in fp64.  The detector takes them into the key 
 (ops.accumulate_sweeps).
 
 evaluation() scores the detections against the infos' objects with evaluate_waymo.waymo_metrics, each box's LEVEL_2
-decided by the label's num_points as the Waymo devkit does.  The devkit's protobuf file is not written."""
+decided by the label's num_points as the Waymo devkit does.  The devkit's protobuf file is not written.  waymo_matching
+(not a reference argument) picks evaluate_waymo's matching: "greedy" (default) or "hungarian"."""
 import os
 
 import numpy as np
@@ -23,13 +24,15 @@ CLASS_NAMES = ["vehicle", "pedestrian", "cyclist"]
 class WaymoDataset(BaseDataset):
     def __init__(self, info_path, root_path, nsweeps, drop_frames=0, sampler=None, loading_pipelines=None,
                  augmentation=None, prepare_label=None, tasks=[], evaluations=None, create_database=False,
-                 use_gt_sampling=True):
+                 use_gt_sampling=True, waymo_matching="greedy"):
         super().__init__(root_path, info_path, sampler, loading_pipelines, augmentation, prepare_label, evaluations,
                          create_database, use_gt_sampling=use_gt_sampling)
         self.nsweeps = nsweeps
         assert self.nsweeps > 0, "At least input one sweep please!"
         self.drop_frames = drop_frames
         assert 0 <= drop_frames <= 1
+        from pillarnext_b200.evaluate_waymo import check_matching
+        self.waymo_matching = check_matching(waymo_matching)
         self.tasks = tasks
 
     def read_file(self, path, timestamp=0):
@@ -77,4 +80,4 @@ class WaymoDataset(BaseDataset):
     def evaluation(self, detections, output_dir=None):
         from pillarnext_b200.evaluate_waymo import waymo_metrics
         class_names = [n for t in self.tasks for n in t] or CLASS_NAMES
-        return waymo_metrics(self.ground_truth(), detections, class_names)
+        return waymo_metrics(self.ground_truth(), detections, class_names, matching=self.waymo_matching)

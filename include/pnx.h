@@ -494,6 +494,52 @@ int pnx_eval_match_host(const float* det_boxes, const float* det_trig, long long
                         const float* gt_trig, int B, int M, int C, const float* thresholds, int* match, float* iou,
                         float* heading);
 
+/* The maximum-IoU (Hungarian) matching of evaluate_waymo.py's matching="hungarian", in three passes.
+ * pnx_eval_pairs: the feasible pairs (IoU >= thresholds[c], the IoU of pnx_eval_match) of every segment, operands as for
+ *   pnx_eval_match.  With edge_start null it writes edge_count [B C] only; with edge_start [B C] (the exclusive prefix
+ *   sum of edge_count) it writes segment s's pairs at [edge_start[s], ..): e_det = detection index, e_box = f M + j,
+ *   e_iou, e_head = the pair's heading accuracy (as pnx_eval_match's); detections in visit order, each one's boxes in
+ *   ascending j.
+ * pnx_eval_components: the connected components of each segment's pairs (E = n_edges).  root [E] = the component's
+ *   first pair; for a root, comp_start [E] = where its pairs begin in grouped [E] (pair indices, each component's
+ *   contiguous, in pair order) and comp_nedge [E] = their number; for any other pair -1 and 0.
+ * pnx_eval_assign: every listed component solved exactly for each breakdown b (0 = all pairs, 1 = pairs whose
+ *   detection and box share a range: det_range [D], gt_range [B M]) and each score cutoff k < K (a detection takes part
+ *   if k < det_pass[d]).  small_roots [n_small] = the roots of the components of at most pnx_eval_assign_warp_pairs()
+ *   pairs (one warp each, shared memory); large_roots [n_large] = the others, large_off [n_large] int64 = the exclusive
+ *   prefix sum of their pair counts, large_pairs = the total.  The assignment maximises the sum of the fp32 IoUs (exact in 40-bit fixed point, every IoU being >=
+ *   2^-17); of several maxima it takes the one chosen detection by detection in visit order, each taking the first
+ *   possible of its boxes in ascending j, then "unmatched".  match [2, K, D] int32 = the box index j within the frame or
+ *   -1, heading [2, K, D] fp32 = the matched pair's e_head or 0.  `workspace` holds
+ *   pnx_eval_assign_workspace(large_pairs) bytes of device memory (no initialisation needed).
+ * All three run on `stream` with no host sync; the _host twins take HOST memory and no workspace. */
+int pnx_eval_pairs(const float* det_boxes, const float* det_trig, long long n_det, const long long* order,
+                   const int* seg_start, const int* seg_count, const float* gt_boxes, const int* gt_classes,
+                   const float* gt_trig, int B, int M, int C, const float* thresholds, const int* edge_start,
+                   int* edge_count, int* e_det, int* e_box, float* e_iou, float* e_head, cudaStream_t stream);
+int pnx_eval_pairs_host(const float* det_boxes, const float* det_trig, long long n_det, const long long* order,
+                        const int* seg_start, const int* seg_count, const float* gt_boxes, const int* gt_classes,
+                        const float* gt_trig, int B, int M, int C, const float* thresholds, const int* edge_start,
+                        int* edge_count, int* e_det, int* e_box, float* e_iou, float* e_head);
+int pnx_eval_components(const int* edge_start, const int* edge_count, int B, int M, int C, long long n_edges,
+                        const int* e_det, const int* e_box, int* root, int* comp_start, int* comp_nedge, int* grouped,
+                        cudaStream_t stream);
+int pnx_eval_components_host(const int* edge_start, const int* edge_count, int B, int M, int C, long long n_edges,
+                             const int* e_det, const int* e_box, int* root, int* comp_start, int* comp_nedge,
+                             int* grouped);
+long long pnx_eval_assign_workspace(long long large_pairs);
+int pnx_eval_assign_warp_pairs(void);
+int pnx_eval_assign(long long n_edges, const int* grouped, const int* comp_start, const int* comp_nedge,
+                    const int* e_det, const int* e_box, const float* e_iou, const float* e_head, const int* small_roots,
+                    int n_small, const int* large_roots, const long long* large_off, int n_large, long long large_pairs,
+                    long long n_det, const int* det_pass, const int* det_range, const int* gt_range, int M, int K,
+                    int* match, float* heading, void* workspace, cudaStream_t stream);
+int pnx_eval_assign_host(long long n_edges, const int* grouped, const int* comp_start, const int* comp_nedge,
+                         const int* e_det, const int* e_box, const float* e_iou, const float* e_head,
+                         const int* small_roots, int n_small, const int* large_roots, const long long* large_off,
+                         int n_large, long long large_pairs, long long n_det, const int* det_pass, const int* det_range,
+                         const int* gt_range, int M, int K, int* match, float* heading);
+
 /* ------------------------------------------------ nuScenes detection score (pillarnext_b200/evaluate_nuscenes.py)
  * pnx_eval_match_center: the centre-distance match of the nuScenes detection benchmark, per (frame, class) segment
  *   s = f C + c and per distance threshold.  det_boxes [n_det, 9] (x, y first); order [n_det] int64 = detection indices

@@ -106,13 +106,22 @@ _SIGS = {
     "pnx_eval_count_points_host": [P, L, I, P, P, P, I, I, P],
     "pnx_eval_match": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P, P],
     "pnx_eval_match_host": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P],
+    # the Hungarian mode: feasible pairs, their connected components, the exact assignment per breakdown and cutoff
+    "pnx_eval_pairs": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P, P, P, P, P],
+    "pnx_eval_pairs_host": [P, P, L, P, P, P, P, P, P, I, I, I, P, P, P, P, P, P, P],
+    "pnx_eval_components": [P, P, I, I, I, L, P, P, P, P, P, P, P],
+    "pnx_eval_components_host": [P, P, I, I, I, L, P, P, P, P, P, P],
+    "pnx_eval_assign_workspace": [L],
+    "pnx_eval_assign_warp_pairs": [],
+    "pnx_eval_assign": [L, P, P, P, P, P, P, P, P, I, P, P, I, L, L, P, P, P, I, I, P, P, P, P],
+    "pnx_eval_assign_host": [L, P, P, P, P, P, P, P, P, I, P, P, I, L, L, P, P, P, I, I, P, P],
     # nuScenes detection score: the centre-distance match, per threshold
     "pnx_eval_match_center": [P, L, P, P, P, P, P, I, I, I, P, I, P, P],
     "pnx_eval_match_center_host": [P, L, P, P, P, P, P, I, I, I, P, I, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,
-            "pnx_accumulate_sweeps_workspace": ctypes.c_longlong,
+            "pnx_accumulate_sweeps_workspace": ctypes.c_longlong, "pnx_eval_assign_workspace": ctypes.c_longlong,
             "pnx_det_iou_bev_host": ctypes.c_float, "pnx_aligned_iou3d_host": ctypes.c_float}
 
 

@@ -17,10 +17,22 @@
 //                          lane computes the fp64 centre distance of the detection to its boxes once, and one shuffle
 //                          arg-min per threshold picks the nearest unmatched box, ties to the lower box index; the match
 //                          holds if that distance is strictly below the threshold.
+//   pnx_eval_pairs         the Hungarian mode's first pass, laid out like pnx_eval_match: one warp per segment writes
+//                          every pair with IoU >= threshold, a ballot compacting each detection's boxes in index order
+//                          (a count pass, then a write pass at the prefix-summed offsets).
+//   pnx_eval_components    one warp per segment; lane 0 joins the pairs sharing a detection or a box (union-find, the
+//                          first pair of a component is its root) and lays each component's pairs out contiguously.
+//   pnx_eval_assign        the exact maximum-IoU assignment of each component per (breakdown, score cutoff): the
+//                          O(N^3) shortest-augmenting-path Hungarian method on the square problem with an "unmatched"
+//                          column per detection and row per box, in 40-bit fixed-point integers, then the tie rule by
+//                          re-solving with the earlier choices fixed wherever the duals leave an option open.  One warp
+//                          and shared memory per (component, breakdown, cutoff) up to kSmallEdges pairs; one CTA and a
+//                          global workspace per larger component.  The same template runs the host twin.
 // The IoU is the reference's boxes_iou3d_gpu arithmetic (box_geom.cuh det_aligned_iou3d_t) with
 // each box's (cos, sin) of the yaw supplied by the caller, so the kernels, their host twins and the CPU oracle see the
 // same trigonometry.  This file is compiled with -fmad=false (pillarnext_b200/build.py): no multiply-add is
 // contracted, so the device results equal the host twins' to the bit.  No host synchronisation inside.
+#include <limits.h>
 #include <math.h>
 
 #include "box_geom.cuh"
@@ -272,6 +284,455 @@ int check_center_args(const CenterArgs& a) {
   return PNX_OK;
 }
 
+// ---------------------------------------------------------------- maximum-IoU assignment (the Hungarian mode)
+constexpr int kSmallEdges = 32;              // components with at most this many feasible pairs: one warp, shared memory
+constexpr int kLargeThreads = 256;           // larger components: one CTA, global workspace
+constexpr long long kInf = LLONG_MAX;        // "no finite reduced cost yet"
+constexpr double kFix = 1099511627776.0;     // 2^40: an fp32 IoU >= 2^-17 is an exact multiple of 2^-40
+
+struct PairArgs {
+  MatchArgs m;                // inputs as for the greedy match; match / iou / heading unused
+  const int* edge_start;      // [B C] or null: count only
+  int* edge_count;            // [B C]
+  int* e_det;                 // [E] detection index
+  int* e_box;                 // [E] f M + j
+  float* e_iou;               // [E]
+  float* e_head;              // [E] heading accuracy of the pair (heading_accuracy, as the greedy match)
+};
+
+// One warp per (frame, class) segment: the detection's IoU against each of the class's boxes (the greedy match's pair
+// routine), and every pair with IoU >= threshold in (detection in visit order, ascending box index) order.
+__global__ void __launch_bounds__(32) eval_pairs_kernel(PairArgs p) {
+  extern __shared__ float smem[];
+  const MatchArgs& a = p.m;
+  const int s = blockIdx.x, lane = threadIdx.x;
+  const int f = s / a.C, c = s - f * a.C;
+  float* rec = smem;
+  int* idx = (int*)(rec + (size_t)a.M * kSlot);
+  const int G = warp_class_boxes(a.gt_classes + (long long)f * a.M, a.M, c, lane, idx);
+  __syncwarp();
+  for (int q = lane; q < G; q += 32) {
+    const long long k = (long long)f * a.M + idx[q];
+    eval_box(a.gt_boxes + k * 9, a.gt_trig + 2 * k, rec + (size_t)q * kSlot);
+  }
+  __syncwarp();
+  const float thr = a.thresholds[c];
+  const int n = a.seg_count[s], base = a.seg_start[s];
+  int cursor = p.edge_start ? p.edge_start[s] : 0;
+  for (int t = 0; t < n; ++t) {
+    const long long di = a.order[base + t];
+    float d[kSlot];
+    eval_box(a.det_boxes + di * 9, a.det_trig + 2 * di, d);
+    for (int q0 = 0; q0 < G; q0 += 32) {
+      const int q = q0 + lane;
+      const float v = q < G ? eval_pair_iou(d, rec + (size_t)q * kSlot) : 0.0f;
+      const bool hit = q < G && v >= thr;
+      const unsigned bal = __ballot_sync(0xffffffffu, hit);
+      if (hit && p.edge_start) {
+        const int e = cursor + __popc(bal & ((1u << lane) - 1u));
+        p.e_det[e] = (int)di;
+        p.e_box[e] = f * a.M + idx[q];
+        p.e_iou[e] = v;
+        p.e_head[e] = heading_accuracy(d[6], rec[(size_t)q * kSlot + 6]);
+      }
+      cursor += __popc(bal);
+    }
+  }
+  if (lane == 0 && !p.edge_start) p.edge_count[s] = cursor;
+}
+
+inline void host_pairs(const PairArgs& p) {
+  const MatchArgs& a = p.m;
+  float* rec = new float[(size_t)(a.M > 0 ? a.M : 1) * kSlot];
+  int* idx = new int[a.M > 0 ? a.M : 1];
+  for (long long s = 0; s < (long long)a.B * a.C; ++s) {
+    const int f = (int)(s / a.C), c = (int)(s % a.C);
+    const int G = host_class_boxes(a.gt_classes + (long long)f * a.M, a.M, c, idx);
+    for (int q = 0; q < G; ++q) {
+      const long long k = (long long)f * a.M + idx[q];
+      eval_box(a.gt_boxes + k * 9, a.gt_trig + 2 * k, rec + (size_t)q * kSlot);
+    }
+    int cursor = p.edge_start ? p.edge_start[s] : 0;
+    for (int t = 0; t < a.seg_count[s]; ++t) {
+      const long long di = a.order[a.seg_start[s] + t];
+      float d[kSlot];
+      eval_box(a.det_boxes + di * 9, a.det_trig + 2 * di, d);
+      for (int q = 0; q < G; ++q) {
+        const float v = eval_pair_iou(d, rec + (size_t)q * kSlot);
+        if (!(v >= a.thresholds[c])) continue;
+        if (p.edge_start) {
+          p.e_det[cursor] = (int)di;
+          p.e_box[cursor] = f * a.M + idx[q];
+          p.e_iou[cursor] = v;
+          p.e_head[cursor] = heading_accuracy(d[6], rec[(size_t)q * kSlot + 6]);
+        }
+        ++cursor;
+      }
+    }
+    if (!p.edge_start) p.edge_count[s] = cursor;
+  }
+  delete[] rec;
+  delete[] idx;
+}
+
+// Union-find over edge ids with the smaller root winning, so each component's root is its first edge.
+__host__ __device__ inline int uf_find(int* parent, int e) {
+  while (parent[e] != e) {
+    parent[e] = parent[parent[e]];
+    e = parent[e];
+  }
+  return e;
+}
+
+__host__ __device__ inline void uf_union(int* parent, int a, int b) {
+  a = uf_find(parent, a);
+  b = uf_find(parent, b);
+  if (a < b) parent[b] = a;
+  else if (b < a) parent[a] = b;
+}
+
+// The connected components of one segment's feasible graph, edges [e0, e1): two edges are joined when they share a
+// detection (consecutive edges, as the pair pass writes them) or a box (last[] = the latest edge of each box, -1 on
+// entry and on exit).  root[e] = the component's first edge; for a root, comp_start = where its edges begin in grouped
+// and comp_nedge = how many there are (components in root order, each one's edges in edge order); otherwise -1 and 0.
+__host__ __device__ inline void segment_components(int e0, int e1, int M, const int* e_det, const int* e_box, int* last,
+                                                   int* root, int* comp_start, int* comp_nedge, int* grouped) {
+  for (int e = e0; e < e1; ++e) {
+    root[e] = e;
+    comp_start[e] = -1;
+    comp_nedge[e] = 0;
+  }
+  for (int e = e0; e < e1; ++e) {
+    if (e > e0 && e_det[e] == e_det[e - 1]) uf_union(root, e, e - 1);
+    const int j = e_box[e] % M;
+    if (last[j] >= 0) uf_union(root, e, last[j]);
+    last[j] = e;
+  }
+  for (int e = e0; e < e1; ++e) {
+    root[e] = uf_find(root, e);
+    ++comp_nedge[root[e]];
+  }
+  int pos = e0;
+  for (int e = e0; e < e1; ++e)
+    if (root[e] == e) { comp_start[e] = pos; pos += comp_nedge[e]; }
+  for (int e = e0; e < e1; ++e) grouped[comp_start[root[e]]++] = e;
+  for (int e = e0; e < e1; ++e) {
+    if (root[e] == e) comp_start[e] -= comp_nedge[e];
+    last[e_box[e] % M] = -1;
+  }
+}
+
+struct CompArgs {
+  const int* edge_start;      // [B C]
+  const int* edge_count;      // [B C]
+  int B, M, C;
+  const int* e_det;
+  const int* e_box;
+  int* root;                  // [E]
+  int* comp_start;            // [E]
+  int* comp_nedge;            // [E]
+  int* grouped;               // [E]
+};
+
+// One warp per segment: the lanes clear the box table, lane 0 walks the segment's edges (a handful per segment).
+__global__ void __launch_bounds__(32) eval_components_kernel(CompArgs a) {
+  extern __shared__ int last[];                               // [M]
+  const int s = blockIdx.x;
+  for (int j = threadIdx.x; j < a.M; j += 32) last[j] = -1;
+  __syncwarp();
+  if (threadIdx.x == 0 && a.edge_count[s] > 0)
+    segment_components(a.edge_start[s], a.edge_start[s] + a.edge_count[s], a.M, a.e_det, a.e_box, last, a.root,
+                       a.comp_start, a.comp_nedge, a.grouped);
+}
+
+struct AssignArgs {
+  const int* grouped;         // [E]
+  const int* comp_start;      // [E]
+  const int* comp_nedge;      // [E]
+  const int* e_det;           // [E]
+  const int* e_box;           // [E]
+  const float* e_iou;         // [E]
+  const float* e_head;        // [E]
+  const int* small_roots;     // [n_small] roots of the components of at most kSmallEdges pairs
+  const int* large_roots;     // [n_large] roots of the larger ones
+  const long long* large_off; // [n_large] exclusive prefix sum of the larger components' pair counts
+  int n_small, n_large;
+  long long E, D, L;          // L = pairs in the larger components
+  const int* det_pass;        // [D] number of score cutoffs the detection passes
+  const int* det_range;       // [D]
+  const int* gt_range;        // [B M]
+  int M, K;
+  int* match;                 // [2, K, D]
+  float* heading;             // [2, K, D]
+  void* workspace;
+};
+
+// One component's state.  Edge arrays hold n_e entries; node arrays (square problem of N = n_d + n_g rows and columns,
+// 1-based as in the textbook O(N^3) Hungarian method) hold N + 1 <= n_e + 2.
+struct CompMem {
+  int *col, *row_start, *row_det, *col_box, *fixed, *p, *way, *pb;
+  long long *w, *u, *v, *minv, *ub, *vb;
+  unsigned char *act, *used;
+  int* scal;                  // [2] n_d, n_g
+};
+
+struct HostGroup {
+  int tid() const { return 0; }
+  int size() const { return 1; }
+  bool leader() const { return true; }
+  void sync() const {}
+  void argmin(long long&, int&) const {}
+};
+
+template <int T>
+struct DevGroup {
+  long long* sv;              // [T / 32] shared scratch of the arg-min
+  int* sj;
+  __device__ int tid() const { return threadIdx.x; }
+  __device__ int size() const { return T; }
+  __device__ bool leader() const { return threadIdx.x == 0; }
+  __device__ void sync() const { __syncthreads(); }
+  // every thread gets the minimum value and, among equal values, the lowest index
+  __device__ void argmin(long long& v, int& j) const {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const long long ov = __shfl_xor_sync(0xffffffffu, v, off);
+      const int oj = __shfl_xor_sync(0xffffffffu, j, off);
+      if (ov < v || (ov == v && oj < j)) { v = ov; j = oj; }
+    }
+    if (T > 32) {
+      if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = v; sj[threadIdx.x >> 5] = j; }
+      __syncthreads();
+      for (int k = 0; k < T / 32; ++k)
+        if (sv[k] < v || (sv[k] == v && sj[k] < j)) { v = sv[k]; j = sj[k]; }
+      __syncthreads();
+    }
+  }
+};
+
+// Cost of square entry (i, j), false if forbidden.  Rows 1..n_d are the detections (visit order), rows n_d+1..N stand
+// for "box j unmatched"; columns 1..n_g are the boxes (ascending index), columns n_g+1..N stand for "detection i
+// unmatched".  A detection row costs -w on its active edges and 0 on its own unmatched column; a box row costs 0 on its
+// own box and on every detection's unmatched column.  fixed[i] != 0 restricts row i to that column.
+__host__ __device__ inline bool lap_cost(const CompMem& m, int n_d, int n_g, int i, int j, long long* c) {
+  if (i <= n_d) {
+    const int f = m.fixed[i];
+    if (f && f != j) return false;
+    if (j > n_g) {
+      *c = 0;
+      return j - n_g == i;
+    }
+    for (int l = m.row_start[i - 1]; l < m.row_start[i] && m.col[l] <= j - 1; ++l)
+      if (m.col[l] == j - 1) {
+        *c = -m.w[l];
+        return m.act[l] != 0;
+      }
+    return false;
+  }
+  *c = 0;
+  return j > n_g || i - n_d == j;
+}
+
+// Minimum-cost perfect assignment of the square problem (successive shortest paths with potentials u, v): p[j] = the
+// row of column j.  Returns the total weight of the detection-box pairs (the maximum total IoU, fixed point), or -1 if
+// the constraints leave no assignment.  Integer arithmetic: the result is the same on every thread count.
+template <class G>
+__host__ __device__ long long lap_solve(const G& g, const CompMem& m, int n_d, int n_g) {
+  const int N = n_d + n_g;
+  for (int j = g.tid(); j <= N; j += g.size()) { m.u[j] = 0; m.v[j] = 0; m.p[j] = 0; m.way[j] = 0; }
+  g.sync();
+  for (int i = 1; i <= N; ++i) {
+    if (g.leader()) m.p[0] = i;
+    for (int j = g.tid(); j <= N; j += g.size()) { m.minv[j] = kInf; m.used[j] = 0; }
+    g.sync();
+    int j0 = 0;
+    for (;;) {
+      if (g.leader()) m.used[j0] = 1;
+      g.sync();
+      const int i0 = m.p[j0];
+      long long best = kInf;
+      int bj = kNone;
+      for (int j = 1 + g.tid(); j <= N; j += g.size()) {
+        if (m.used[j]) continue;
+        long long c;
+        if (lap_cost(m, n_d, n_g, i0, j, &c)) {
+          const long long cur = c - m.u[i0] - m.v[j];
+          if (cur < m.minv[j]) { m.minv[j] = cur; m.way[j] = j0; }
+        }
+        if (m.minv[j] < best) { best = m.minv[j]; bj = j; }
+      }
+      g.argmin(best, bj);
+      g.sync();
+      if (bj == kNone || best == kInf) return -1;
+      // read before the barrier: the update loop does not write p, the leader's augmentation after the break does
+      const bool free_col = m.p[bj] == 0;
+      for (int j = g.tid(); j <= N; j += g.size()) {
+        if (m.used[j]) { m.u[m.p[j]] += best; m.v[j] -= best; }
+        else if (m.minv[j] != kInf) m.minv[j] -= best;
+      }
+      g.sync();
+      j0 = bj;
+      if (free_col) break;
+    }
+    if (g.leader()) {
+      do {
+        const int j1 = m.way[j0];
+        m.p[j0] = m.p[j1];
+        j0 = j1;
+      } while (j0);
+    }
+    g.sync();
+  }
+  long long total = 0;
+  for (int j = 1; j <= n_g; ++j) {
+    long long c;
+    if (m.p[j] <= n_d && lap_cost(m, n_d, n_g, m.p[j], j, &c)) total -= c;
+  }
+  g.sync();
+  return total;
+}
+
+// The tie rule: of all maximum-IoU assignments, the one chosen detection by detection in visit order, each taking the
+// first still possible of its active boxes in ascending index, then "unmatched".  An option is possible when some
+// optimal assignment agrees with every earlier choice and with it; an option off the current duals' tight set is not,
+// the current assignment's own is, and any other is decided by solving again with it fixed.
+template <class G>
+__host__ __device__ void lex_assign(const G& g, const CompMem& m, int n_d, int n_g) {
+  const int N = n_d + n_g;
+  for (int i = g.tid(); i <= n_d; i += g.size()) m.fixed[i] = 0;
+  g.sync();
+  const long long V = lap_solve(g, m, n_d, n_g);
+  for (int i = 1; i <= n_d; ++i) {
+    int cc = 0;
+    for (int j = 1; j <= N; ++j)
+      if (m.p[j] == i) cc = j;
+    int l = m.row_start[i - 1];
+    const int l1 = m.row_start[i];
+    for (;;) {
+      while (l < l1 && !m.act[l]) ++l;
+      const int o = l < l1 ? m.col[l++] + 1 : n_g + i;
+      if (o == cc) break;
+      if (o <= n_g && m.p[o] >= 1 && m.p[o] < i) continue;        // held by an earlier, fixed detection
+      long long c;
+      lap_cost(m, n_d, n_g, i, o, &c);
+      if (c - m.u[i] - m.v[o] == 0) {
+        for (int j = g.tid(); j <= N; j += g.size()) { m.ub[j] = m.u[j]; m.vb[j] = m.v[j]; m.pb[j] = m.p[j]; }
+        if (g.leader()) m.fixed[i] = o;
+        g.sync();
+        if (lap_solve(g, m, n_d, n_g) == V) { cc = o; break; }
+        for (int j = g.tid(); j <= N; j += g.size()) { m.u[j] = m.ub[j]; m.v[j] = m.vb[j]; m.p[j] = m.pb[j]; }
+        if (g.leader()) m.fixed[i] = 0;
+        g.sync();
+      }
+      if (o > n_g) break;                                         // unreachable: the current column is an option
+    }
+    if (g.leader()) m.fixed[i] = cc;
+    g.sync();
+  }
+}
+
+// Loads component `root` for (mode, cutoff kc): rows (its detections in visit order), columns (its boxes in ascending
+// index), edge weights and which edges are active -- the detection passes cutoff kc and, in mode 1, lies in the box's
+// range.  Returns (n_d, n_g) through m.scal.
+template <class G>
+__host__ __device__ void load_component(const G& g, const AssignArgs& a, int root, const CompMem& m, int mode, int kc) {
+  const int start = a.comp_start[root], n_e = a.comp_nedge[root];
+  const int* ge = a.grouped + start;
+  for (int l = g.tid(); l < n_e; l += g.size()) {
+    const int k = a.e_box[ge[l]];
+    bool first = true;
+    for (int q = 0; q < l && first; ++q) first = a.e_box[ge[q]] != k;
+    m.used[l] = first;
+  }
+  g.sync();
+  for (int l = g.tid(); l < n_e; l += g.size()) {
+    const int e = ge[l], k = a.e_box[e], det = a.e_det[e];
+    int c = 0;
+    for (int q = 0; q < n_e; ++q) c += m.used[q] && a.e_box[ge[q]] < k;
+    m.col[l] = c;
+    if (m.used[l]) m.col_box[c] = k;
+    m.w[l] = (long long)((double)a.e_iou[e] * kFix);
+    m.act[l] = kc < a.det_pass[det] && (mode == 0 || a.det_range[det] == a.gt_range[k]);
+  }
+  if (g.leader()) {
+    int n_d = 0, n_g = 0;
+    for (int l = 0; l < n_e; ++l) {
+      n_g += m.used[l];
+      if (l == 0 || a.e_det[ge[l]] != a.e_det[ge[l - 1]]) { m.row_det[n_d] = a.e_det[ge[l]]; m.row_start[n_d++] = l; }
+    }
+    m.row_start[n_d] = n_e;
+    m.scal[0] = n_d;
+    m.scal[1] = n_g;
+  }
+  g.sync();
+}
+
+template <class G>
+__host__ __device__ void assign_component(const G& g, const AssignArgs& a, int root, const CompMem& m, int mode,
+                                          int kc) {
+  load_component(g, a, root, m, mode, kc);
+  const int n_d = m.scal[0], n_g = m.scal[1];
+  lex_assign(g, m, n_d, n_g);
+  const long long at = ((long long)mode * a.K + kc) * a.D;
+  const int* ge = a.grouped + a.comp_start[root];
+  for (int i = 1 + g.tid(); i <= n_d; i += g.size()) {
+    const int f = m.fixed[i], det = m.row_det[i - 1];
+    float h = 0.0f;
+    for (int l = m.row_start[i - 1]; l < m.row_start[i]; ++l)
+      if (m.col[l] == f - 1) h = a.e_head[ge[l]];
+    a.match[at + det] = f <= n_g ? m.col_box[f - 1] % a.M : -1;
+    a.heading[at + det] = h;
+  }
+  g.sync();
+}
+
+// Components of at most kSmallEdges pairs, one warp per (component, breakdown, cutoff), all state in shared memory.
+__global__ void __launch_bounds__(32) eval_assign_small_kernel(AssignArgs a) {
+  constexpr int kE = kSmallEdges, kN = kSmallEdges + 2;
+  __shared__ int col[kE], row_start[kE + 1], row_det[kE], col_box[kE], fixed[kE + 1], p[kN], way[kN], pb[kN], scal[2];
+  __shared__ long long w[kE], u[kN], v[kN], minv[kN], ub[kN], vb[kN];
+  __shared__ unsigned char act[kE], used[kN];
+  const int root = a.small_roots[blockIdx.x];
+  const CompMem m{col, row_start, row_det, col_box, fixed, p, way, pb, w, u, v, minv, ub, vb, act, used, scal};
+  assign_component(DevGroup<32>{nullptr, nullptr}, a, root, m, blockIdx.y / a.K, blockIdx.y % a.K);
+}
+
+// Offsets of one component's state in the global workspace: every array is 2L long (L = the pairs of all the larger
+// components), the component's at twice its large_off (n_e > kSmallEdges >= 2 pairs, so 2 n_e >= n_e + 2 covers the node
+// arrays).
+__host__ __device__ inline CompMem workspace_mem(void* ws, long long E, long long at, int* scal) {
+  long long* L = (long long*)ws;
+  int* I = (int*)(L + 6 * 2 * E);
+  unsigned char* U = (unsigned char*)(I + 8 * 2 * E);
+  const long long n = 2 * E;
+  return CompMem{I + at, I + n + at, I + 2 * n + at, I + 3 * n + at, I + 4 * n + at, I + 5 * n + at, I + 6 * n + at,
+                 I + 7 * n + at, L + at, L + n + at, L + 2 * n + at, L + 3 * n + at, L + 4 * n + at, L + 5 * n + at,
+                 U + at, U + n + at, scal};
+}
+
+long long assign_workspace_bytes(long long E) { return 2 * E * (6 * 8 + 8 * 4 + 2); }
+
+// Components of more than kSmallEdges pairs: one CTA each, every breakdown and cutoff in turn, state in the workspace.
+__global__ void __launch_bounds__(kLargeThreads) eval_assign_large_kernel(AssignArgs a) {
+  __shared__ long long sv[kLargeThreads / 32];
+  __shared__ int sj[kLargeThreads / 32], scal[2];
+  const int root = a.large_roots[blockIdx.x];
+  const CompMem m = workspace_mem(a.workspace, a.L, 2 * a.large_off[blockIdx.x], scal);
+  for (int y = 0; y < 2 * a.K; ++y) assign_component(DevGroup<kLargeThreads>{sv, sj}, a, root, m, y / a.K, y % a.K);
+}
+
+int check_assign_args(const AssignArgs& a) {
+  PNX_CHECK_ARG(a.E >= 0 && a.E < (1LL << 30) && a.D >= 0 && a.D < (1LL << 31), "number of pairs / detections");
+  PNX_CHECK_ARG(a.K >= 1 && a.K <= 1024 && a.M >= 1, "1 to 1024 score cutoffs, M >= 1");
+  PNX_CHECK_ARG(a.E == 0 || (a.grouped && a.comp_start && a.comp_nedge && a.e_det && a.e_box && a.e_iou && a.e_head &&
+                              a.gt_range), "pair pointers");
+  PNX_CHECK_ARG(a.n_small >= 0 && a.n_large >= 0 && (long long)a.n_small + a.n_large <= a.E && a.L >= 0 && a.L <= a.E,
+                "component lists");
+  PNX_CHECK_ARG(a.n_small == 0 || a.small_roots, "small_roots");
+  PNX_CHECK_ARG(a.n_large == 0 || (a.large_roots && a.large_off), "large_roots / large_off");
+  PNX_CHECK_ARG(a.D == 0 || (a.det_pass && a.det_range && a.match && a.heading), "detection pointers");
+  return PNX_OK;
+}
 
 }  // namespace
 
@@ -428,5 +889,144 @@ extern "C" int pnx_eval_match_center_host(const float* det_boxes, long long n_de
   }
   delete[] idx;
   delete[] used;
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_pairs(const float* det_boxes, const float* det_trig, long long n_det, const long long* order,
+                              const int* seg_start, const int* seg_count, const float* gt_boxes, const int* gt_classes,
+                              const float* gt_trig, int B, int M, int C, const float* thresholds, const int* edge_start,
+                              int* edge_count, int* e_det, int* e_box, float* e_iou, float* e_head, cudaStream_t stream) {
+  const PairArgs p{{det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, B, M, C, thresholds,
+                    nullptr, nullptr, nullptr},
+                   edge_start, edge_count, e_det, e_box, e_iou, e_head};
+  PNX_CHECK_ARG(n_det >= 0 && n_det < (1LL << 31), "number of detections");
+  PNX_CHECK_ARG(B == 0 || (edge_start ? (e_det && e_box && e_iou && e_head) : edge_count != nullptr), "pair outputs");
+  const MatchArgs& a = p.m;
+  const int nd = (int)n_det;
+  PNX_CHECK_ARG(a.B >= 0 && a.C >= 1 && a.M >= 0 && a.M <= kMaxBoxesPerFrame, "B / C / at most 4096 boxes per frame");
+  PNX_CHECK_ARG((long long)a.B * a.C < (1LL << 31), "too many segments");
+  PNX_CHECK_ARG(nd == 0 || (a.det_boxes && a.det_trig && a.order), "detection pointers");
+  PNX_CHECK_ARG((long long)a.B * a.M == 0 || (a.gt_boxes && a.gt_classes && a.gt_trig), "ground-truth pointers");
+  PNX_CHECK_ARG(a.B == 0 || (a.seg_start && a.seg_count && a.thresholds), "segment / threshold pointers");
+  if (B == 0) return PNX_OK;
+  const size_t smem = (size_t)M * (kSlot * sizeof(float) + sizeof(int));
+  if (smem > 48 * 1024) PNX_CUDA(cudaFuncSetAttribute(eval_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  eval_pairs_kernel<<<B * C, 32, smem, stream>>>(p);
+  PNX_CHECK_LAUNCH();
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_pairs_host(const float* det_boxes, const float* det_trig, long long n_det, const long long* order,
+                                   const int* seg_start, const int* seg_count, const float* gt_boxes, const int* gt_classes,
+                                   const float* gt_trig, int B, int M, int C, const float* thresholds,
+                                   const int* edge_start, int* edge_count, int* e_det, int* e_box, float* e_iou, float* e_head) {
+  const PairArgs p{{det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, B, M, C, thresholds,
+                    nullptr, nullptr, nullptr},
+                   edge_start, edge_count, e_det, e_box, e_iou, e_head};
+  PNX_CHECK_ARG(n_det >= 0 && n_det < (1LL << 31), "number of detections");
+  PNX_CHECK_ARG(B == 0 || (edge_start ? (e_det && e_box && e_iou && e_head) : edge_count != nullptr), "pair outputs");
+  const MatchArgs& a = p.m;
+  PNX_CHECK_ARG(a.B >= 0 && a.C >= 1 && a.M >= 0 && a.M <= kMaxBoxesPerFrame, "B / C / at most 4096 boxes per frame");
+  PNX_CHECK_ARG((long long)a.B * a.C < (1LL << 31), "too many segments");
+  PNX_CHECK_ARG(n_det == 0 || (a.det_boxes && a.det_trig && a.order), "detection pointers");
+  PNX_CHECK_ARG((long long)a.B * a.M == 0 || (a.gt_boxes && a.gt_classes && a.gt_trig), "ground-truth pointers");
+  PNX_CHECK_ARG(a.B == 0 || (a.seg_start && a.seg_count && a.thresholds), "segment / threshold pointers");
+  host_pairs(p);
+  return PNX_OK;
+}
+
+static int check_comp_args(const CompArgs& a, long long n_edges) {
+  PNX_CHECK_ARG(a.B >= 0 && a.C >= 1 && a.M >= 0 && a.M <= kMaxBoxesPerFrame, "B / C / at most 4096 boxes per frame");
+  PNX_CHECK_ARG((long long)a.B * a.C < (1LL << 31) && n_edges >= 0 && n_edges < (1LL << 30), "segments / pairs");
+  PNX_CHECK_ARG(a.B == 0 || (a.edge_start && a.edge_count), "segment pointers");
+  PNX_CHECK_ARG(n_edges == 0 || (a.e_det && a.e_box && a.root && a.comp_start && a.comp_nedge && a.grouped),
+                "pair pointers");
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_components(const int* edge_start, const int* edge_count, int B, int M, int C, long long n_edges,
+                                   const int* e_det, const int* e_box, int* root, int* comp_start, int* comp_nedge,
+                                   int* grouped, cudaStream_t stream) {
+  const CompArgs a{edge_start, edge_count, B, M, C, e_det, e_box, root, comp_start, comp_nedge, grouped};
+  int rc = check_comp_args(a, n_edges);
+  if (rc) return rc;
+  if (n_edges == 0) return PNX_OK;
+  eval_components_kernel<<<B * C, 32, (size_t)M * sizeof(int), stream>>>(a);
+  PNX_CHECK_LAUNCH();
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_components_host(const int* edge_start, const int* edge_count, int B, int M, int C,
+                                        long long n_edges, const int* e_det, const int* e_box, int* root,
+                                        int* comp_start, int* comp_nedge, int* grouped) {
+  const CompArgs a{edge_start, edge_count, B, M, C, e_det, e_box, root, comp_start, comp_nedge, grouped};
+  int rc = check_comp_args(a, n_edges);
+  if (rc) return rc;
+  if (n_edges == 0) return PNX_OK;
+  int* last = new int[M];
+  for (int j = 0; j < M; ++j) last[j] = -1;
+  for (long long s = 0; s < (long long)B * C; ++s)
+    if (edge_count[s] > 0)
+      segment_components(edge_start[s], edge_start[s] + edge_count[s], M, e_det, e_box, last, root, comp_start,
+                         comp_nedge, grouped);
+  delete[] last;
+  return PNX_OK;
+}
+
+extern "C" long long pnx_eval_assign_workspace(long long large_pairs) { return assign_workspace_bytes(large_pairs); }
+
+extern "C" int pnx_eval_assign_warp_pairs(void) { return kSmallEdges; }
+
+extern "C" int pnx_eval_assign(long long n_edges, const int* grouped, const int* comp_start, const int* comp_nedge,
+                               const int* e_det, const int* e_box, const float* e_iou, const float* e_head,
+                               const int* small_roots, int n_small, const int* large_roots, const long long* large_off,
+                               int n_large, long long large_pairs, long long n_det, const int* det_pass,
+                               const int* det_range, const int* gt_range, int M, int K, int* match, float* heading,
+                               void* workspace, cudaStream_t stream) {
+  const AssignArgs a{grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, small_roots, large_roots, large_off,
+                     n_small, n_large, n_edges, n_det, large_pairs, det_pass, det_range, gt_range, M, K, match, heading,
+                     workspace};
+  int rc = check_assign_args(a);
+  if (rc) return rc;
+  PNX_CHECK_ARG(n_large == 0 || workspace, "workspace");
+  PNX_CHECK_ARG(2 * K <= 65535, "at most 32767 score cutoffs on the device");
+  if (n_det > 0) {
+    PNX_CUDA(cudaMemsetAsync(match, 0xff, (size_t)2 * K * n_det * sizeof(int), stream));
+    PNX_CUDA(cudaMemsetAsync(heading, 0, (size_t)2 * K * n_det * sizeof(float), stream));
+  }
+  if (n_small > 0) {
+    eval_assign_small_kernel<<<dim3((unsigned)n_small, 2 * K), 32, 0, stream>>>(a);
+    PNX_CHECK_LAUNCH();
+  }
+  if (n_large > 0) {
+    eval_assign_large_kernel<<<(unsigned)n_large, kLargeThreads, 0, stream>>>(a);
+    PNX_CHECK_LAUNCH();
+  }
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_assign_host(long long n_edges, const int* grouped, const int* comp_start, const int* comp_nedge,
+                                    const int* e_det, const int* e_box, const float* e_iou, const float* e_head,
+                                    const int* small_roots, int n_small, const int* large_roots,
+                                    const long long* large_off, int n_large, long long large_pairs, long long n_det,
+                                    const int* det_pass, const int* det_range, const int* gt_range, int M, int K,
+                                    int* match, float* heading) {
+  const AssignArgs a{grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, small_roots, large_roots, large_off,
+                     n_small, n_large, n_edges, n_det, large_pairs, det_pass, det_range, gt_range, M, K, match, heading,
+                     nullptr};
+  int rc = check_assign_args(a);
+  if (rc) return rc;
+  for (long long i = 0; i < 2 * K * n_det; ++i) { match[i] = -1; heading[i] = 0.0f; }
+  // every component through the same state layout, one at a time: one region sized for kSmallEdges + 2 or the largest
+  long long cap = kSmallEdges + 2;
+  for (int r = 0; r < n_large; ++r) cap = comp_nedge[large_roots[r]] > cap ? comp_nedge[large_roots[r]] : cap;
+  void* ws = new char[assign_workspace_bytes(cap)];
+  int scal[2];
+  for (int r = 0; r < n_small + n_large; ++r) {
+    const int root = r < n_small ? small_roots[r] : large_roots[r - n_small];
+    const CompMem m = workspace_mem(ws, cap, 0, scal);
+    for (int y = 0; y < 2 * K; ++y) assign_component(HostGroup{}, a, root, m, y / K, y % K);
+  }
+  delete[] (char*)ws;
   return PNX_OK;
 }

@@ -1212,6 +1212,151 @@ def eval_match_host(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, 
     return match, iou, heading
 
 
+def eval_pairs(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, thresholds):
+    """The feasible pairs (IoU >= the class threshold) of every (frame, class) segment (pnx_eval_pairs, include/pnx.h),
+    operands as for eval_match, all CUDA -> (edge_start [B C] int32, e_det [E] int32 detection index, e_box [E] int32
+    f M + j, e_iou [E] fp32, e_head [E] fp32 heading accuracy as eval_match's), each segment's pairs from edge_start
+    on.  One count pass, one prefix sum, one host read of E, one write pass."""
+    db, dt, od, ss, sc, gb, gc, gt, th = _eval_match_operands(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes,
+                                                              gt_classes, gt_trig, thresholds)
+    D, (B, M), C = len(db), gb.shape[:2], len(th)
+    dev = db.device
+    count = torch.zeros(B * C, dtype=torch.int32, device=dev)
+    args = (ptr(db), ptr(dt), D, ptr(od), ptr(ss), ptr(sc), ptr(gb), ptr(gc), ptr(gt), B, M, C, ptr(th))
+    _count(2)
+    check(lib().pnx_eval_pairs(*args, None, ptr(count), None, None, None, None, stream()))
+    end = torch.cumsum(count, 0, dtype=torch.int64)
+    E = int(end[-1]) if B * C else 0
+    start = (end - count).to(torch.int32)
+    e_det, e_box = (torch.empty(E, dtype=torch.int32, device=dev) for _ in range(2))
+    e_iou, e_head = (torch.empty(E, dtype=torch.float32, device=dev) for _ in range(2))
+    if E:
+        check(lib().pnx_eval_pairs(*args, ptr(start), ptr(count), ptr(e_det), ptr(e_box), ptr(e_iou), ptr(e_head),
+                                   stream()))
+    return start, e_det, e_box, e_iou, e_head
+
+
+def eval_pairs_host(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes, gt_classes, gt_trig, thresholds):
+    """Host twin of eval_pairs (pnx_eval_pairs_host): the same operands as numpy arrays -> the same five arrays."""
+    db, dt, od, ss, sc, gb, gc, gt, th = _eval_match_operands(det_boxes, det_trig, order, seg_start, seg_count, gt_boxes,
+                                                              gt_classes, gt_trig, thresholds, host=True)
+    D, (B, M), C = len(db), gb.shape[:2], len(th)
+    count = np.zeros(B * C, np.int32)
+    args = (_hp(db), _hp(dt), D, _hp(od), _hp(ss), _hp(sc), _hp(gb), _hp(gc), _hp(gt), B, M, C, _hp(th))
+    check(lib().pnx_eval_pairs_host(*args, None, _hp(count), None, None, None, None))
+    start = (np.cumsum(count, dtype=np.int64) - count).astype(np.int32)
+    E = int(count.sum(dtype=np.int64))
+    e_det, e_box = np.zeros(E, np.int32), np.zeros(E, np.int32)
+    e_iou, e_head = np.zeros(E, np.float32), np.zeros(E, np.float32)
+    if E:
+        check(lib().pnx_eval_pairs_host(*args, _hp(start), _hp(count), _hp(e_det), _hp(e_box), _hp(e_iou), _hp(e_head)))
+    return start, e_det, e_box, e_iou, e_head
+
+
+def _eval_components_operands(edge_start, e_det, e_box, host=False):
+    E = len(e_det)
+    i32 = torch.int32
+    return [_want(t, i32, shape, what, host) for t, shape, what in (
+        (edge_start, (len(edge_start),), "edge_start"), (e_det, (E,), "e_det"), (e_box, (E,), "e_box"))]
+
+
+def _edge_count(start, E):
+    """Pairs per segment from the segments' first pair and the total E."""
+    if isinstance(start, np.ndarray):
+        return (np.append(start[1:], E) - start).astype(np.int32)
+    return (torch.cat([start[1:], start.new_full((1,), E)]) - start).to(torch.int32)
+
+
+def eval_components(edge_start, e_det, e_box, M, n_classes):
+    """Connected components of each segment's feasible pairs (pnx_eval_components, include/pnx.h), all CUDA:
+    edge_start [B C] int32 and e_det / e_box [E] int32 of eval_pairs, M boxes per frame, C = n_classes ->
+    (comp_start [E] int32, comp_nedge [E] int32, grouped [E] int32): for each component's first pair, where its pairs
+    begin in grouped and how many there are; -1 and 0 for every other pair."""
+    st, ed, eb = _eval_components_operands(edge_start, e_det, e_box)
+    E, C = len(ed), int(n_classes)
+    B = len(st) // C
+    count = _edge_count(st, E)
+    root, comp_start, comp_nedge, grouped = (torch.empty(E, dtype=torch.int32, device=ed.device) for _ in range(4))
+    _count(1)
+    check(lib().pnx_eval_components(ptr(st), ptr(count), B, int(M), C, E, ptr(ed), ptr(eb), ptr(root), ptr(comp_start),
+                                    ptr(comp_nedge), ptr(grouped), stream()))
+    return comp_start, comp_nedge, grouped
+
+
+def eval_components_host(edge_start, e_det, e_box, M, n_classes):
+    """Host twin of eval_components (pnx_eval_components_host): numpy in, numpy out."""
+    st, ed, eb = _eval_components_operands(edge_start, e_det, e_box, host=True)
+    E, C = len(ed), int(n_classes)
+    B = len(st) // C
+    count = _edge_count(st, E)
+    root, comp_start, comp_nedge, grouped = (np.zeros(E, np.int32) for _ in range(4))
+    check(lib().pnx_eval_components_host(_hp(st), _hp(count), B, int(M), C, E, _hp(ed), _hp(eb), _hp(root),
+                                         _hp(comp_start), _hp(comp_nedge), _hp(grouped)))
+    return comp_start, comp_nedge, grouped
+
+
+def _eval_assign_operands(grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, det_pass, det_range, gt_range,
+                          host=False):
+    E, D = len(e_det), len(det_pass)
+    f32, i32 = torch.float32, torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (grouped, i32, (E,), "grouped"), (comp_start, i32, (E,), "comp_start"), (comp_nedge, i32, (E,), "comp_nedge"),
+        (e_det, i32, (E,), "e_det"), (e_box, i32, (E,), "e_box"), (e_iou, f32, (E,), "e_iou"),
+        (e_head, f32, (E,), "e_head"), (det_pass, i32, (D,), "det_pass"), (det_range, i32, (D,), "det_range"),
+        (gt_range, i32, (len(gt_range),), "gt_range"))]
+
+
+def _component_lists(comp_nedge, xp):
+    """Roots of the components the one-warp solver takes, roots of the larger ones, the larger ones' exclusive prefix
+    sum of pairs (their workspace offsets) and their total.  xp = torch or numpy."""
+    warp = lib().pnx_eval_assign_warp_pairs()
+    if xp is torch:
+        small = torch.nonzero((comp_nedge > 0) & (comp_nedge <= warp)).view(-1).to(torch.int32)
+        large = torch.nonzero(comp_nedge > warp).view(-1)
+        n = comp_nedge[large].to(torch.int64)
+        end = torch.cumsum(n, 0)
+        return small, large.to(torch.int32), end - n, int(end[-1]) if len(n) else 0
+    small = np.nonzero((comp_nedge > 0) & (comp_nedge <= warp))[0].astype(np.int32)
+    large = np.nonzero(comp_nedge > warp)[0]
+    n = comp_nedge[large].astype(np.int64)
+    return small, large.astype(np.int32), np.cumsum(n) - n, int(n.sum())
+
+
+def eval_assign(grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, det_pass, det_range, gt_range, M, K):
+    """Maximum-IoU assignment of every component, per breakdown and score cutoff (pnx_eval_assign, include/pnx.h), all
+    CUDA: the pairs and components of eval_pairs / eval_components, det_pass [D] int32 (cutoffs each detection passes),
+    det_range [D] and gt_range [B M] int32 range bins, M, K cutoffs -> (match [2, K, D] int32, the box index within the
+    frame or -1; heading [2, K, D] fp32, the matched pair's e_head or 0), breakdown 0: all pairs; 1: pairs within one
+    range bin.  The components are listed by size on the device (one host read of the counts), and only the larger
+    ones get workspace."""
+    ops_ = _eval_assign_operands(grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, det_pass, det_range,
+                                 gt_range)
+    E, D = len(ops_[3]), len(ops_[7])
+    dev = ops_[7].device
+    small, large, large_off, large_pairs = _component_lists(ops_[2], torch)
+    match = torch.empty((2, int(K), D), dtype=torch.int32, device=dev)
+    heading = torch.empty((2, int(K), D), dtype=torch.float32, device=dev)
+    ws = torch.empty(max(1, lib().pnx_eval_assign_workspace(large_pairs)), dtype=torch.uint8, device=dev)
+    _count(2)
+    check(lib().pnx_eval_assign(E, *[ptr(t) for t in ops_[:7]], ptr(small), len(small), ptr(large), ptr(large_off),
+                                len(large), large_pairs, D, *[ptr(t) for t in ops_[7:]], int(M), int(K), ptr(match),
+                                ptr(heading), ptr(ws), stream()))
+    return match, heading
+
+
+def eval_assign_host(grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, det_pass, det_range, gt_range, M, K):
+    """Host twin of eval_assign (pnx_eval_assign_host): numpy in -> (match [2, K, D] int32, heading [2, K, D] fp32)."""
+    ops_ = _eval_assign_operands(grouped, comp_start, comp_nedge, e_det, e_box, e_iou, e_head, det_pass, det_range,
+                                 gt_range, host=True)
+    E, D = len(ops_[3]), len(ops_[7])
+    small, large, large_off, large_pairs = _component_lists(ops_[2], np)
+    match, heading = np.zeros((2, int(K), D), np.int32), np.zeros((2, int(K), D), np.float32)
+    check(lib().pnx_eval_assign_host(E, *[_hp(t) for t in ops_[:7]], _hp(small), len(small), _hp(large),
+                                     _hp(large_off), len(large), large_pairs, D, *[_hp(t) for t in ops_[7:]], int(M),
+                                     int(K), _hp(match), _hp(heading)))
+    return match, heading
+
+
 # --------------------------------------------------------------------------------- nuScenes detection score
 def _eval_match_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, dist_ths,
                                 host=False):

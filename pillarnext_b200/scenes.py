@@ -188,11 +188,13 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
 
     metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map), "waymo" (evaluate_waymo.waymo_metrics,
     AP / APH at LEVEL_1 and LEVEL_2) or "nds" (evaluate_nuscenes.nuscenes_metrics, the nuScenes detection score with
-    its true-positive errors).  For "waymo" and "nds" ground_truth() also hands over each frame's points."""
+    its true-positive errors).  For "waymo" and "nds" ground_truth() also hands over each frame's points.
+    waymo_matching: for metric "waymo", "greedy" (the default) or "hungarian" (the maximum-IoU matching at score-cutoff
+    quantiles with the range breakdown, evaluate_waymo.py)."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
                  augmentation=None, sampler=None, root_path=None, metric="nuscenes", nsweeps=1, drop_frames=0.0,
-                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, **_):
+                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, waymo_matching="greedy", **_):
         if int(nsweeps) < 1 or not 0.0 <= drop_frames <= 1.0 or min_distance < 0:
             raise ValueError("nsweeps must be >= 1, drop_frames in [0, 1] and min_distance >= 0, got %r, %r, %r"
                              % (nsweeps, drop_frames, min_distance))
@@ -203,6 +205,8 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         if metric not in ("nuscenes", "waymo", "nds"):
             raise ValueError("metric must be 'nuscenes', 'waymo' or 'nds', got %r" % (metric,))
         self.metric = metric
+        from .evaluate_waymo import check_matching
+        self.waymo_matching = check_matching(waymo_matching)
         self.class_names = [n for t in cfg["tasks"] for n in t]
         if augmentation and test_mode:
             raise ValueError("augmentation is a training transform: a test_mode dataset must not set it")
@@ -260,7 +264,7 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         """The hook the reference trainer calls at the end of val_epoch (base.py:48-51, trainer.py:165-184)."""
         if self.metric == "waymo":
             from .evaluate_waymo import waymo_metrics
-            return waymo_metrics(self.ground_truth(), detections, self.class_names)
+            return waymo_metrics(self.ground_truth(), detections, self.class_names, matching=self.waymo_matching)
         if self.metric == "nds":
             from .evaluate_nuscenes import nuscenes_metrics
             return nuscenes_metrics(self.ground_truth(), detections, self.class_names)
