@@ -37,11 +37,16 @@ struct Rows {  // a split row matrix: piece q of channel c at p[m*ld + q*lo + c]
 __device__ __forceinline__ void load_split8(const Rows& r, long long m, int c0, float (&f)[8]) {
   // smallest piece first: the partial sums are exact in fp32 (pieces are non-overlapping 8-bit windows of one fp32)
   unpack8(*reinterpret_cast<const uint4*>(r.p + m * r.ld + (r.pieces - 1) * r.lo + c0), f);
+  float g[8];
   for (int q = r.pieces - 2; q >= 0; --q) {
-    float g[8];
     unpack8(*reinterpret_cast<const uint4*>(r.p + m * r.ld + q * r.lo + c0), g);
 #pragma unroll
     for (int k = 0; k < 8; ++k) f[k] += g[k];
+  }
+  // a zero sum takes the sign of piece 0 (now in g): -0 splits into -0, +0, ..., whose fp32 sum is +0
+  if (r.pieces > 1) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = f[k] == 0.f ? copysignf(0.f, g[k]) : f[k];
   }
 }
 __device__ __forceinline__ void store_split8(const Rows& r, long long m, int c0, const float (&f)[8]) {

@@ -8,7 +8,9 @@ that every product and every fp32 partial sum is exact in any summation order: f
 equal the fp64 reference, bf16 outputs the fp64 reference rounded to bf16, bit for bit.  At these shapes a CTA walks
 tens to hundreds of tiles, which the kernel tests' small shapes never make it do.  Everything else a launch writes is
 checked too: guard columns and rows past M keep a sentinel, BatchNorm statistics (both accumulation modes) and the fused
-BatchNorm-backward reduce match fp64 sums.  A configuration the replay cannot reproduce fails the test."""
+BatchNorm-backward reduce match fp64 sums.  A configuration the replay cannot reproduce fails the test.  The split
+mode's configurations (segments over bf16 pieces) are replayed through the same functions by
+tests/test_production_split_gpu.py."""
 import types
 
 import pytest
@@ -272,8 +274,9 @@ def _gemm_view(c):
 
 
 def _amplitudes(c):
-    """(A, W, bias, addend) integer amplitudes; the largest possible |partial sum| must stay below 2^24."""
-    k = c["taps"] * c["cin"] if c["kind"] == "igemm" else 9 * c["cin"]
+    """(A, W, bias, addend) integer amplitudes; the largest possible |partial sum| must stay below 2^24.  A split-mode
+    GEMM accumulates its nseg segments into one accumulator: K counts every segment."""
+    k = (c["taps"] * c["cin"] if c["kind"] == "igemm" else 9 * c["cin"]) * len(c.get("segs") or (None,))
     for a, w in ((3, 2), (2, 2), (1, 2), (1, 1)):
         bound = k * a * w + 4 + 8
         if bound < EXACT:
@@ -281,18 +284,46 @@ def _amplitudes(c):
     raise Unreproducible("K = %d: no integer range keeps the sums exact" % k)
 
 
+def seg_pieces(c):
+    """(A pieces, W pieces) a configuration reads: 1, 1 for a plain GEMM, 3, 3 for a 3-piece split-mode one."""
+    segs = c.get("segs") or ((0, 0),)
+    return max(a for a, _ in segs) + 1, max(w for _, w in segs) + 1
+
+
+def pieces_buffer(desc, cols, lo, pieces, amp, gen):
+    """_rows_buffer for split rows: its own integers in the columns [q lo, q lo + cols) of every piece q, NaN between
+    the pieces and past the last (a piece offset that is off reads NaN or another piece's integers).  One NaN row past
+    the view, so a reference taken at a shifted piece offset stays inside the storage."""
+    shape, stride, dt = desc
+    if len(shape) != 2 or stride[1] != 1 or stride[0] < shape[1] or lo < cols or (pieces - 1) * lo + cols > shape[1]:
+        raise Unreproducible("split operand layout %s for %d pieces of %d columns at %d" % (desc, pieces, cols, lo))
+    buf = torch.full((shape[0] + 1, stride[0]), float("nan"), dtype=dt, device="cuda")
+    for q in range(pieces):
+        buf[:shape[0], q * lo:q * lo + cols] = _ints((shape[0], cols), amp, buf.dtype, gen)
+    return buf[:shape[0], :shape[1]]
+
+
+def piece(t, off, cols):
+    """Columns [off, off + cols) of every row of the row-major view t, read through its storage (off may pass the view)."""
+    return t.as_strided((t.shape[0], cols), (t.stride(0), 1), t.storage_offset() + off)
+
+
 def _gemm_operands(c, gen, tables):
-    if c["kind"] == "igemm" and (c["segs"] or c["a_lo_off"]):
-        raise Unreproducible("split-mode segments")
+    if c["kind"] == "igemm" and c["a_lo_off"] and not c["segs"]:
+        raise Unreproducible("a piece offset without segments")
     if c["overlap"]:
         raise Unreproducible("operands share elements")
     g = _gemm_view(c)
     (aa, aw, ab, ad), bound = _amplitudes(c)
     assert bound < EXACT
     o = types.SimpleNamespace(bound=bound)
-    o.A = _rows_buffer(c["A"], g["cin"], aa, gen)
+    a_pieces, w_pieces = seg_pieces(c)
+    # split mode: no valid split (its low pieces would be zero, and a wrong piece offset would go unnoticed); every
+    # piece of A and of W holds its own integers
+    o.A = _rows_buffer(c["A"], g["cin"], aa, gen) if a_pieces == 1 else \
+        pieces_buffer(c["A"], g["cin"], c["a_lo_off"], a_pieces, aa, gen)
     wshape = c["W"] if c["kind"] == "igemm" else c["W_"]
-    if tuple(wshape) != (g["taps"], g["cout"], g["cin"]):
+    if tuple(wshape) != (g["taps"], g["cout"], w_pieces * g["cin"]):
         raise Unreproducible("packed weight shape %s" % (wshape,))
     o.W = _ints(wshape, aw, torch.bfloat16, gen)
     o.bias = _ints((g["cout"],), ab, torch.float32, gen) if c["bias"] else None
@@ -319,21 +350,31 @@ def _launch_gemm(c, o):
     if c["kind"] == "igemm":
         ops.igemm(o.A, c["M"], o.W, c["taps"], c["cin"], c["cout"], o.out, lda=c["lda"], ldc=c["ldc"], nbr=o.table, dense=c["dense"],
                   bias=o.bias, stats=stats, stats_mod=c["stats_mod"], shuffle=c["shuffle"], relu=c["relu"], block_n=c["bn"],
-                  addend=o.addend, bnr=o.bnr)
+                  addend=o.addend, segs=c["segs"], a_lo_off=c["a_lo_off"], bnr=o.bnr)
     else:
         ops.conv3x3_win(o.A, c["B"], c["H"], c["W"], o.W, c["cin"], c["cout"], o.out, bias=o.bias, stats=stats, relu=c["relu"],
                         block_n=c["bn"], base_off=c["base_off"], bnr=o.bnr)
     return stats, (o.bnr.red.clone() if o.bnr is not None else None)
 
 
-def _gemm_reference(c, o, drop=None, bias_delta=None, skip_tile=None):
-    """fp64 reference of the stored output (in the output dtype), the stats sums and the bnr sums.  The mutations exist to
-    show that the comparison notices them: drop = (row, tap) whose gather is left out, bias_delta = (column, delta),
-    skip_tile = a 128-row tile left out of the statistics."""
+def _gemm_reference(c, o, drop=None, bias_delta=None, skip_tile=None, segs=None, a_lo_off=None):
+    """fp64 reference of the stored output (in the output dtype), the stats sums and the bnr sums.  A split-mode
+    configuration sums, over its segments (A piece ap, W piece wp), gathered piece ap of A times piece wp of W.  The
+    mutations exist to show that the comparison notices them: drop = (row, tap) whose gather is left out, bias_delta =
+    (column, delta), skip_tile = a 128-row tile left out of the statistics, segs / a_lo_off in place of the recorded ones."""
     g = _gemm_view(c)
     M, taps, cin, cout = g["M"], g["taps"], g["cin"], g["cout"]
     dev = o.A.device
+    segs = c.get("segs") if segs is None else segs
+    lo = c.get("a_lo_off", 0) if a_lo_off is None else a_lo_off
     Wd = o.W.double()
+    if segs:               # the W pieces each A piece meets, summed (exact: small integers)
+        groups = {}
+        for ap, wp in segs:
+            groups[ap] = groups.get(ap, 0) + Wd[:, :, wp * cin:(wp + 1) * cin]
+        terms = [(piece(o.A, ap * lo, cin), w) for ap, w in sorted(groups.items())]
+    else:
+        terms = [(o.A, Wd)]
     bias = o.bias.double() if o.bias is not None else None
     if bias is not None and bias_delta is not None:
         bias = bias.clone()
@@ -354,7 +395,8 @@ def _gemm_reference(c, o, drop=None, bias_delta=None, skip_tile=None):
             if drop is not None and m0 <= drop[0] < m1 and t == drop[1]:
                 idx = idx.clone()
                 idx[drop[0] - m0] = -1
-            v += _gather(o.A, idx, cin) @ Wd[t].t()
+            for src, w in terms:
+                v += _gather(src, idx, cin) @ w[t].t()
         if bias is not None:
             v += bias
         if o.addend is not None:

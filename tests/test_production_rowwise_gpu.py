@@ -100,15 +100,19 @@ EXCLUDED = {
 
 # ------------------------------------------------------------------------------------------------- recording
 class Recorder:
-    """The library handle's proxy: keeps one record per unique configuration of the ARG_MAPS entry points."""
+    """The library handle's proxy: keeps one record per unique configuration of the entry points in `maps` (default
+    ARG_MAPS); `extra(name)`, when given, adds fields of the library's state at the call to the configuration."""
 
-    def __init__(self, real):
+    def __init__(self, real, maps=None, extra=None):
         self.real, self.configs, self.keys, self.called, self.source = real, [], {}, set(), ""
+        self.maps, self.extra = ARG_MAPS if maps is None else maps, extra
 
     def _add(self, name, args):
-        spec = arg_map(name)
+        spec = [tuple(a.split(":")) for a in self.maps[name].split()]
         assert len(args) == len(spec), (name, len(args))
         cfg = {"fn": name}
+        if self.extra is not None:
+            cfg.update(self.extra(name))
         for (arg, kind), v in zip(spec, args):
             if arg == "stream":
                 continue
@@ -135,7 +139,7 @@ class Recorder:
                 if not name.startswith("pnx_"):
                     return fn
                 rec.called.add(name)
-                if name not in ARG_MAPS:
+                if name not in rec.maps:
                     return fn
 
                 def call(*args):
@@ -863,16 +867,17 @@ def _stencil_gather_ref(Z, bias, B, H, W, cpt, drop=None):
     return out
 
 
-def _stencil_scatter_ref(dout, B, H, W, nz, cpt):
-    """dZ[m, (3r + s) cpt + j] = bf16(dout[(y - r + 1, x - s + 1), j]) inside the image, else 0; columns >= 9 cpt zero."""
+def _stencil_scatter_ref(dout, B, H, W, nz, cpt, dtype=torch.bfloat16):
+    """dZ[m, (3r + s) cpt + j] = bf16(dout[(y - r + 1, x - s + 1), j]) inside the image, else 0; columns >= 9 cpt zero.
+    dtype = torch.float32: the values before the rounding."""
     M = B * H * W
-    dZ = torch.zeros(M, nz, dtype=torch.bfloat16, device=dout.device)
+    dZ = torch.zeros(M, nz, dtype=dtype, device=dout.device)
     for b in range(B):
         Dp = F.pad(dout[b * H * W:(b + 1) * H * W, :cpt].reshape(H, W, cpt).permute(2, 0, 1), (1, 1, 1, 1))
         rows = dZ[b * H * W:(b + 1) * H * W]
         for t in range(9):
             r, s = t // 3, t % 3
-            rows[:, t * cpt:(t + 1) * cpt] = Dp[:, 2 - r:2 - r + H, 2 - s:2 - s + W].permute(1, 2, 0).reshape(H * W, cpt).bfloat16()
+            rows[:, t * cpt:(t + 1) * cpt] = Dp[:, 2 - r:2 - r + H, 2 - s:2 - s + W].permute(1, 2, 0).reshape(H * W, cpt).to(dtype)
     return dZ
 
 
