@@ -10,7 +10,13 @@ transform inv(pose) @ sweep_pose in fp64.  The detector takes them into the key 
 
 evaluation() scores the detections against the infos' objects with evaluate_waymo.waymo_metrics, each box's LEVEL_2
 decided by the label's num_points as the Waymo devkit does.  The devkit's protobuf file is not written.  waymo_matching
-(not a reference argument) picks evaluate_waymo's matching: "greedy" (default) or "hungarian"."""
+(not a reference argument) picks evaluate_waymo's matching: "greedy" (default) or "hungarian".
+
+tracking=True (not a reference argument) also tracks the detections through each sequence (pillarnext_b200.track, the
+sequence and timestamp split from the token "<context_name>-<timestamp_micros>" as the reference's evaluation() does,
+the frame's pose from the info) and scores the tracks with evaluate_waymo_tracking.waymo_tracking_metrics; the result
+gains "tracking" (those metrics) and "tracks" (token -> the detection's dict plus "tracking_id").  ground_truth() then
+also carries each object's "ids" and the frame's "sequence", "timestamp" and "pose".  Off, both are unchanged."""
 import os
 
 import numpy as np
@@ -24,7 +30,7 @@ CLASS_NAMES = ["vehicle", "pedestrian", "cyclist"]
 class WaymoDataset(BaseDataset):
     def __init__(self, info_path, root_path, nsweeps, drop_frames=0, sampler=None, loading_pipelines=None,
                  augmentation=None, prepare_label=None, tasks=[], evaluations=None, create_database=False,
-                 use_gt_sampling=True, waymo_matching="greedy"):
+                 use_gt_sampling=True, waymo_matching="greedy", tracking=False):
         super().__init__(root_path, info_path, sampler, loading_pipelines, augmentation, prepare_label, evaluations,
                          create_database, use_gt_sampling=use_gt_sampling)
         self.nsweeps = nsweeps
@@ -34,6 +40,7 @@ class WaymoDataset(BaseDataset):
         from pillarnext_b200.evaluate_waymo import check_matching
         self.waymo_matching = check_matching(waymo_matching)
         self.tasks = tasks
+        self.tracking = bool(tracking)
 
     def read_file(self, path, timestamp=0):
         points = np.fromfile(os.path.join(self._root_path, path), dtype=np.float32).reshape(-1, 6)
@@ -75,9 +82,19 @@ class WaymoDataset(BaseDataset):
             gts[info["token"]] = {"boxes": np.array([o["box"] for o in objs], np.float32).reshape(-1, 9),
                                   "names": [o["label"] for o in objs],
                                   "num_points": np.array([o["num_points"] for o in objs], np.int64)}
+            if self.tracking:
+                from pillarnext_b200.track import split_token
+                seq, ts = split_token(info["token"])
+                gts[info["token"]].update(ids=[o["id"] for o in objs], sequence=seq, timestamp=ts,
+                                          pose=np.asarray(info["pose"], np.float64))
         return gts
 
     def evaluation(self, detections, output_dir=None):
         from pillarnext_b200.evaluate_waymo import waymo_metrics
         class_names = [n for t in self.tasks for n in t] or CLASS_NAMES
-        return waymo_metrics(self.ground_truth(), detections, class_names, matching=self.waymo_matching)
+        gts = self.ground_truth()
+        res = waymo_metrics(gts, detections, class_names, matching=self.waymo_matching)
+        if self.tracking:
+            from pillarnext_b200.evaluate_waymo_tracking import track_and_score
+            res["tracks"], res["tracking"] = track_and_score(gts, detections, class_names)
+        return res

@@ -540,6 +540,58 @@ int pnx_eval_assign_host(long long n_edges, const int* grouped, const int* comp_
                          int n_large, long long large_pairs, long long n_det, const int* det_pass, const int* det_range,
                          const int* gt_range, int M, int K, int* match, float* heading);
 
+/* ------------------------------------------------ tracking (pillarnext_b200/track.py, evaluate_waymo_tracking.py)
+ * pnx_track_greedy: the velocity-based greedy tracker, per (sequence, class).  boxes [n_det, 9] fp32 (x, y, z, dx, dy,
+ *   dz, vx, vy, yaw in the frame's sensor coordinates), scores [n_det]; order [n_det] int64 = detection indices sorted
+ *   by segment f C + c, then descending score, ties to the lower index; segment s holds order[seg_start[s] ..
+ *   + seg_count[s]) ([F C] int32); poses [F, 4, 4] fp64 sensor -> global; times [F] int64 microseconds; the frames of
+ *   sequence q are [seq_start[q], seq_start[q + 1]) ([S + 1] int32), in ascending time; max_dist [C] fp32 metres.
+ *   Per frame, each detection with score >= min_score (in order) takes the unclaimed live track nearest to its
+ *   back-projected global centre p - v dt, if within max_dist (ties to the older track), else starts a track; matched
+ *   tracks take the detection's p and v, the others move by v dt and are dropped after more than max_age misses
+ *   (track.py's docstring states every rounding).  Output track_id [n_det] int64: ids consecutive per sequence in
+ *   birth order (frame, class, visit order), -1 below min_score.  Scratch: local_id [n_det], births [S C], map
+ *   [n_det] int32; row_det_start [S C] int64 = the exclusive prefix sum of the detections per (sequence, class).
+ *   status [1] int32 = 0, or 1 + the first (sequence, class) whose live tracks would exceed cap (its ids are then
+ *   incomplete, the rest -1).  cap in [1, pnx_track_max_tracks()] = the track slots per (sequence, class) in shared
+ *   memory; min(pnx_track_max_tracks(), (max_age + 2) x the largest seg_count) can never run out early, as every live
+ *   track was matched or born in the last max_age + 1 frames, plus this frame's births.  C <= 64.  The host twin takes
+ *   HOST memory, no scratch, and pnx_track_max_tracks() slots.
+ * pnx_eval_mot: the CLEAR-MOT frame matching of evaluate_waymo_tracking.py, one row per (sequence, class, cutoff)
+ *   walking the sequence's frames (seq_start [S + 1], frames as for pnx_eval_pairs' segments).  Inputs: the pairs of
+ *   pnx_eval_pairs (edge_start / edge_count [B C], e_det, e_box, e_iou), the components of pnx_eval_components
+ *   (grouped, comp_start, comp_nedge), det_pass [n_det] (cutoffs each detection passes), det_id [n_det] int32
+ *   tracking ids >= 0, gt_obj [B M] int32 object index in [0, n_obj) or -1, gt_points [B M] int32 point counts.
+ *   Per frame: carry-over (pairs in order whose detection passes the cutoff and carries the object's last matched id,
+ *   each unless its detection or box is already kept), then the tie-ruled maximum-IoU assignment of pnx_eval_assign on
+ *   the remaining pairs.  Outputs counts [S, C, K, 5] int64 = matches (every level), L1 matches, L1 mismatches, L2
+ *   matches, L2 mismatches (L1: > 5 points, L2: >= 1), dist [S, C, K, 2] fp64 = the sum of 1 - IoU over the L1 / L2
+ *   matches in match order, last_id [K, n_obj] int32 scratch.  cap >= max(pnx_eval_assign_warp_pairs() + 2, the
+ *   largest component's pair count); workspace = pnx_eval_mot_workspace(S C K, M, cap) bytes, about
+ *   S C K (164 cap + 4 M): every row gets room for the largest component anywhere.  The host twin takes
+ *   HOST memory and no workspace. */
+int pnx_track_max_tracks(void);
+int pnx_track_greedy(const float* boxes, const float* scores, long long n_det, const long long* order,
+                     const int* seg_start, const int* seg_count, const double* poses, const long long* times,
+                     const int* seq_start, int S, int F, int C, const float* max_dist, int max_age, float min_score,
+                     int cap, const long long* row_det_start, int* local_id, int* births, int* map,
+                     long long* track_id, int* status, cudaStream_t stream);
+int pnx_track_greedy_host(const float* boxes, const float* scores, long long n_det, const long long* order,
+                          const int* seg_start, const int* seg_count, const double* poses, const long long* times,
+                          const int* seq_start, int S, int F, int C, const float* max_dist, int max_age,
+                          float min_score, long long* track_id, int* status);
+long long pnx_eval_mot_workspace(int rows, int M, int cap);
+int pnx_eval_mot(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                 const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box, const float* e_iou,
+                 long long n_det, const int* det_pass, const int* det_id, const int* gt_obj, const int* gt_points,
+                 const int* seq_start, int S, int B, int M, int C, int K, int n_obj, int cap, int* last_id,
+                 long long* counts, double* dist, void* workspace, cudaStream_t stream);
+int pnx_eval_mot_host(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                      const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box,
+                      const float* e_iou, long long n_det, const int* det_pass, const int* det_id, const int* gt_obj,
+                      const int* gt_points, const int* seq_start, int S, int B, int M, int C, int K, int n_obj, int cap,
+                      int* last_id, long long* counts, double* dist);
+
 /* ------------------------------------------------ nuScenes detection score (pillarnext_b200/evaluate_nuscenes.py)
  * pnx_eval_match_center: the centre-distance match of the nuScenes detection benchmark, per (frame, class) segment
  *   s = f C + c and per distance threshold.  det_boxes [n_det, 9] (x, y first); order [n_det] int64 = detection indices

@@ -115,6 +115,13 @@ _SIGS = {
     "pnx_eval_assign_warp_pairs": [],
     "pnx_eval_assign": [L, P, P, P, P, P, P, P, P, I, P, P, I, L, L, P, P, P, I, I, P, P, P, P],
     "pnx_eval_assign_host": [L, P, P, P, P, P, P, P, P, I, P, P, I, L, L, P, P, P, I, I, P, P],
+    # tracking: the greedy velocity tracker and the CLEAR-MOT frame matching of evaluate_waymo_tracking
+    "pnx_track_max_tracks": [],
+    "pnx_track_greedy": [P, P, L, P, P, P, P, P, P, I, I, I, P, I, F, I, P, P, P, P, P, P, P],
+    "pnx_track_greedy_host": [P, P, L, P, P, P, P, P, P, I, I, I, P, I, F, P, P],
+    "pnx_eval_mot_workspace": [I, I, I],
+    "pnx_eval_mot": [P, P, L, P, P, P, P, P, P, L, P, P, P, P, P, I, I, I, I, I, I, I, P, P, P, P, P],
+    "pnx_eval_mot_host": [P, P, L, P, P, P, P, P, P, L, P, P, P, P, P, I, I, I, I, I, I, I, P, P, P],
     # nuScenes detection score: the centre-distance match, per threshold
     "pnx_eval_match_center": [P, L, P, P, P, P, P, I, I, I, P, I, P, P],
     "pnx_eval_match_center_host": [P, L, P, P, P, P, P, I, I, I, P, I, P],
@@ -122,6 +129,7 @@ _SIGS = {
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,
             "pnx_accumulate_sweeps_workspace": ctypes.c_longlong, "pnx_eval_assign_workspace": ctypes.c_longlong,
+            "pnx_eval_mot_workspace": ctypes.c_longlong,
             "pnx_det_iou_bev_host": ctypes.c_float, "pnx_aligned_iou3d_host": ctypes.c_float}
 
 

@@ -15,8 +15,8 @@ OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
-# det_eval.cu's kernels must equal their host twins to the bit, so no fp32 multiply-add is contracted there
-FILE_FLAGS = {"det_eval.cu": ["-fmad=false"]}
+# det_eval.cu's and track.cu's kernels must equal their host twins to the bit, so no multiply-add is contracted there
+FILE_FLAGS = {"det_eval.cu": ["-fmad=false"], "track.cu": ["-fmad=false"]}
 
 
 def _sources():

@@ -28,6 +28,12 @@
 //                          re-solving with the earlier choices fixed wherever the duals leave an option open.  One warp
 //                          and shared memory per (component, breakdown, cutoff) up to kSmallEdges pairs; one CTA and a
 //                          global workspace per larger component.  The same template runs the host twin.
+//   pnx_eval_mot           the CLEAR-MOT frame matching of evaluate_waymo_tracking.py: one warp per (sequence, class,
+//                          score cutoff) walks the sequence's frames; per frame the leader keeps the pairs that carry
+//                          each object's previous id, then every component is solved by the same tie-ruled assignment
+//                          over the pairs left active, its state in the row's slice of a global workspace, and the
+//                          leader counts matches, mismatches and sum(1 - IoU) per level.  The host twin runs the same
+//                          template one row at a time.
 // The IoU is the reference's boxes_iou3d_gpu arithmetic (box_geom.cuh det_aligned_iou3d_t) with
 // each box's (cos, sin) of the yaw supplied by the caller, so the kernels, their host twins and the CPU oracle see the
 // same trigonometry.  This file is compiled with -fmad=false (pillarnext_b200/build.py): no multiply-add is
@@ -477,11 +483,11 @@ struct CompMem {
 };
 
 struct HostGroup {
-  int tid() const { return 0; }
-  int size() const { return 1; }
-  bool leader() const { return true; }
-  void sync() const {}
-  void argmin(long long&, int&) const {}
+  __host__ __device__ int tid() const { return 0; }
+  __host__ __device__ int size() const { return 1; }
+  __host__ __device__ bool leader() const { return true; }
+  __host__ __device__ void sync() const {}
+  __host__ __device__ void argmin(long long&, int&) const {}
 };
 
 template <int T>
@@ -631,40 +637,54 @@ __host__ __device__ void lex_assign(const G& g, const CompMem& m, int n_d, int n
   }
 }
 
-// Loads component `root` for (mode, cutoff kc): rows (its detections in visit order), columns (its boxes in ascending
-// index), edge weights and which edges are active -- the detection passes cutoff kc and, in mode 1, lies in the box's
-// range.  Returns (n_d, n_g) through m.scal.
-template <class G>
-__host__ __device__ void load_component(const G& g, const AssignArgs& a, int root, const CompMem& m, int mode, int kc) {
-  const int start = a.comp_start[root], n_e = a.comp_nedge[root];
-  const int* ge = a.grouped + start;
+// Loads the component of pairs ge[0 .. n_e): rows (its detections in visit order), columns (its boxes in ascending
+// index), edge weights and which edges are active (active(e, det, box)).  Returns (n_d, n_g) through m.scal.
+template <class G, class Active>
+__host__ __device__ void load_edges(const G& g, const int* ge, int n_e, const int* e_det, const int* e_box,
+                                    const float* e_iou, const CompMem& m, const Active& active) {
   for (int l = g.tid(); l < n_e; l += g.size()) {
-    const int k = a.e_box[ge[l]];
+    const int k = e_box[ge[l]];
     bool first = true;
-    for (int q = 0; q < l && first; ++q) first = a.e_box[ge[q]] != k;
+    for (int q = 0; q < l && first; ++q) first = e_box[ge[q]] != k;
     m.used[l] = first;
   }
   g.sync();
   for (int l = g.tid(); l < n_e; l += g.size()) {
-    const int e = ge[l], k = a.e_box[e], det = a.e_det[e];
+    const int e = ge[l], k = e_box[e], det = e_det[e];
     int c = 0;
-    for (int q = 0; q < n_e; ++q) c += m.used[q] && a.e_box[ge[q]] < k;
+    for (int q = 0; q < n_e; ++q) c += m.used[q] && e_box[ge[q]] < k;
     m.col[l] = c;
     if (m.used[l]) m.col_box[c] = k;
-    m.w[l] = (long long)((double)a.e_iou[e] * kFix);
-    m.act[l] = kc < a.det_pass[det] && (mode == 0 || a.det_range[det] == a.gt_range[k]);
+    m.w[l] = (long long)((double)e_iou[e] * kFix);
+    m.act[l] = active(e, det, k);
   }
   if (g.leader()) {
     int n_d = 0, n_g = 0;
     for (int l = 0; l < n_e; ++l) {
       n_g += m.used[l];
-      if (l == 0 || a.e_det[ge[l]] != a.e_det[ge[l - 1]]) { m.row_det[n_d] = a.e_det[ge[l]]; m.row_start[n_d++] = l; }
+      if (l == 0 || e_det[ge[l]] != e_det[ge[l - 1]]) { m.row_det[n_d] = e_det[ge[l]]; m.row_start[n_d++] = l; }
     }
     m.row_start[n_d] = n_e;
     m.scal[0] = n_d;
     m.scal[1] = n_g;
   }
   g.sync();
+}
+
+// The detection-metric rule: the detection passes cutoff kc and, in mode 1, lies in the box's range.
+struct CutoffRange {
+  const AssignArgs& a;
+  int mode, kc;
+  __host__ __device__ bool operator()(int, int det, int k) const {
+    return kc < a.det_pass[det] && (mode == 0 || a.det_range[det] == a.gt_range[k]);
+  }
+};
+
+// Loads component `root` for (mode, cutoff kc).
+template <class G>
+__host__ __device__ void load_component(const G& g, const AssignArgs& a, int root, const CompMem& m, int mode, int kc) {
+  load_edges(g, a.grouped + a.comp_start[root], a.comp_nedge[root], a.e_det, a.e_box, a.e_iou, m,
+             CutoffRange{a, mode, kc});
 }
 
 template <class G>
@@ -710,7 +730,7 @@ __host__ __device__ inline CompMem workspace_mem(void* ws, long long E, long lon
                  U + at, U + n + at, scal};
 }
 
-long long assign_workspace_bytes(long long E) { return 2 * E * (6 * 8 + 8 * 4 + 2); }
+__host__ __device__ inline long long assign_workspace_bytes(long long E) { return 2 * E * (6 * 8 + 8 * 4 + 2); }
 
 // Components of more than kSmallEdges pairs: one CTA each, every breakdown and cutoff in turn, state in the workspace.
 __global__ void __launch_bounds__(kLargeThreads) eval_assign_large_kernel(AssignArgs a) {
@@ -731,6 +751,140 @@ int check_assign_args(const AssignArgs& a) {
   PNX_CHECK_ARG(a.n_small == 0 || a.small_roots, "small_roots");
   PNX_CHECK_ARG(a.n_large == 0 || (a.large_roots && a.large_off), "large_roots / large_off");
   PNX_CHECK_ARG(a.D == 0 || (a.det_pass && a.det_range && a.match && a.heading), "detection pointers");
+  return PNX_OK;
+}
+
+// ---------------------------------------------------------------- CLEAR-MOT frame matching (evaluate_waymo_tracking.py)
+struct MotArgs {
+  const int* edge_start;      // [B C] first pair of each segment (pnx_eval_pairs)
+  const int* edge_count;      // [B C]
+  const int* grouped;         // [E] components of pnx_eval_components
+  const int* comp_start;      // [E]
+  const int* comp_nedge;      // [E]
+  const int* e_det;           // [E]
+  const int* e_box;           // [E] f M + j
+  const float* e_iou;         // [E]
+  const int* det_pass;        // [D] number of score cutoffs the detection passes
+  const int* det_id;          // [D] tracking id >= 0
+  const int* gt_obj;          // [B M] object index in [0, n_obj), -1 = none
+  const int* gt_points;       // [B M] point count (difficulty level)
+  const int* seq_start;       // [S + 1] the frames of sequence s are [seq_start[s], seq_start[s + 1])
+  int S, B, M, C, K, n_obj, cap;
+  long long E, D;
+  int* last_id;               // [K, n_obj] the tracking id of each object's last match, -1 = none yet
+  long long* counts;          // [S, C, K, 5] matches; L1 matches, L1 mismatches; L2 matches, L2 mismatches
+  double* dist;               // [S, C, K, 2] sum of 1 - IoU over the L1 / L2 matches
+  void* workspace;            // [S C K] x mot_row_bytes(M, cap)
+};
+
+constexpr int kMotCounts = 5;
+
+// one row's workspace: the assignment state of a component of up to cap pairs, then the frame's kept-box table [M]
+__host__ __device__ inline long long mot_comp_bytes(int cap) { return (assign_workspace_bytes(cap) + 15) / 16 * 16; }
+__host__ __device__ inline long long mot_row_bytes(int M, int cap) {
+  return mot_comp_bytes(cap) + ((long long)M * sizeof(int) + 15) / 16 * 16;
+}
+
+// Pairs the assignment may use at cutoff kc: the detection passes it, and neither the detection nor the box was kept
+// by the carry-over (kept[j] = the detection holding box j, -1 = none; a detection's pairs are consecutive in [e0, e1)).
+struct MotActive {
+  const MotArgs& a;
+  const int* kept;
+  int kc, e0, e1;
+  __host__ __device__ bool operator()(int e, int det, int k) const {
+    if (kc >= a.det_pass[det] || kept[k % a.M] >= 0) return false;
+    for (int q = e; q >= e0 && a.e_det[q] == det; --q)
+      if (kept[a.e_box[q] % a.M] == det) return false;
+    for (int q = e + 1; q < e1 && a.e_det[q] == det; ++q)
+      if (kept[a.e_box[q] % a.M] == det) return false;
+    return true;
+  }
+};
+
+// One match (detection det, box kb = f M + j, fp32 IoU): the counts of the levels the box belongs to, a mismatch when
+// the object's previous match carried another id, and the object's last id.  n and d as MotArgs::counts / dist.
+__host__ __device__ inline void mot_count(const MotArgs& a, int* last, int det, int kb, float iou, long long* n,
+                                          double* d) {
+  const int o = a.gt_obj[kb], id = a.det_id[det], pts = a.gt_points[kb];
+  const bool mism = o >= 0 && last[o] >= 0 && last[o] != id;
+  if (o >= 0) last[o] = id;
+  const double miss_iou = 1.0 - (double)iou;
+  ++n[0];
+  if (pts > 5) { ++n[1]; n[2] += mism; d[0] += miss_iou; }
+  if (pts >= 1) { ++n[3]; n[4] += mism; d[1] += miss_iou; }
+}
+
+// One (sequence, class, cutoff) row, frames in order: the carry-over (leader, pairs in order), then every component of
+// the frame's pairs solved by the tie-ruled maximum-IoU assignment over the pairs left active.  Counts on the leader.
+template <class G>
+__host__ __device__ void mot_row(const G& g, const MotArgs& a, int row, const CompMem& m, int* kept) {
+  const int s = row / (a.C * a.K), c = (row / a.K) % a.C, kc = row % a.K;
+  int* last = a.last_id + (long long)kc * a.n_obj;
+  long long n[kMotCounts] = {0, 0, 0, 0, 0};
+  double d[2] = {0.0, 0.0};
+  for (int f = a.seq_start[s]; f < a.seq_start[s + 1]; ++f) {
+    const int seg = f * a.C + c;
+    const int e0 = a.edge_start[seg], e1 = e0 + a.edge_count[seg];
+    for (int e = e0 + g.tid(); e < e1; e += g.size()) kept[a.e_box[e] % a.M] = -1;
+    g.sync();
+    if (g.leader()) {
+      bool det_kept = false;
+      for (int e = e0; e < e1; ++e) {
+        const int det = a.e_det[e], kb = a.e_box[e], j = kb % a.M;
+        if (e > e0 && det != a.e_det[e - 1]) det_kept = false;
+        if (det_kept || kc >= a.det_pass[det] || kept[j] >= 0) continue;
+        const int o = a.gt_obj[kb];
+        if (o < 0 || last[o] != a.det_id[det]) continue;
+        kept[j] = det;
+        det_kept = true;
+        mot_count(a, last, det, kb, a.e_iou[e], n, d);
+      }
+    }
+    g.sync();
+    for (int r = e0; r < e1; ++r) {
+      if (a.comp_start[r] < 0) continue;                       // not a component's first pair
+      const int* ge = a.grouped + a.comp_start[r];
+      load_edges(g, ge, a.comp_nedge[r], a.e_det, a.e_box, a.e_iou, m, MotActive{a, kept, kc, e0, e1});
+      bool any = false;
+      for (int l = 0; l < a.comp_nedge[r]; ++l) any |= m.act[l] != 0;
+      if (!any) continue;
+      const int n_d = m.scal[0], n_g = m.scal[1];
+      lex_assign(g, m, n_d, n_g);
+      if (g.leader())
+        for (int i = 1; i <= n_d; ++i) {
+          const int fx = m.fixed[i];
+          if (fx > n_g) continue;
+          for (int l = m.row_start[i - 1]; l < m.row_start[i]; ++l)
+            if (m.col[l] == fx - 1) { mot_count(a, last, m.row_det[i - 1], a.e_box[ge[l]], a.e_iou[ge[l]], n, d); break; }
+        }
+      g.sync();
+    }
+  }
+  if (g.leader()) {
+    for (int q = 0; q < kMotCounts; ++q) a.counts[(long long)row * kMotCounts + q] = n[q];
+    a.dist[2 * (long long)row] = d[0];
+    a.dist[2 * (long long)row + 1] = d[1];
+  }
+}
+
+// One warp per (sequence, class, cutoff) row, its state in its slice of the workspace.
+__global__ void __launch_bounds__(32) eval_mot_kernel(MotArgs a) {
+  __shared__ int scal[2];
+  char* base = (char*)a.workspace + (long long)blockIdx.x * mot_row_bytes(a.M, a.cap);
+  const CompMem m = workspace_mem(base, a.cap, 0, scal);
+  mot_row(DevGroup<32>{nullptr, nullptr}, a, blockIdx.x, m, (int*)(base + mot_comp_bytes(a.cap)));
+}
+
+int check_mot_args(const MotArgs& a) {
+  PNX_CHECK_ARG(a.S >= 0 && a.B >= 0 && a.C >= 1 && a.K >= 1 && a.n_obj >= 0, "S / B / C / K / n_obj");
+  PNX_CHECK_ARG(a.M >= 1 && a.M <= kMaxBoxesPerFrame, "1 to 4096 boxes per frame");
+  PNX_CHECK_ARG((long long)a.S * a.C * a.K < (1LL << 31) && (long long)a.B * a.C < (1LL << 31), "too many rows");
+  PNX_CHECK_ARG(a.cap >= kSmallEdges + 2, "cap >= pnx_eval_assign_warp_pairs() + 2");
+  PNX_CHECK_ARG(a.E >= 0 && a.E < (1LL << 30) && a.D >= 0 && a.D < (1LL << 31), "number of pairs / detections");
+  PNX_CHECK_ARG(a.seq_start && (a.B == 0 || (a.edge_start && a.edge_count)), "segment pointers");
+  PNX_CHECK_ARG(a.E == 0 || (a.grouped && a.comp_start && a.comp_nedge && a.e_det && a.e_box && a.e_iou &&
+                              a.det_pass && a.det_id && a.gt_obj && a.gt_points), "pair pointers");
+  PNX_CHECK_ARG(a.S == 0 || (a.last_id && a.counts && a.dist), "output pointers");
   return PNX_OK;
 }
 
@@ -1028,5 +1182,45 @@ extern "C" int pnx_eval_assign_host(long long n_edges, const int* grouped, const
     for (int y = 0; y < 2 * K; ++y) assign_component(HostGroup{}, a, root, m, y / K, y % K);
   }
   delete[] (char*)ws;
+  return PNX_OK;
+}
+
+extern "C" long long pnx_eval_mot_workspace(int rows, int M, int cap) { return (long long)rows * mot_row_bytes(M, cap); }
+
+extern "C" int pnx_eval_mot(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                            const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box,
+                            const float* e_iou, long long n_det, const int* det_pass, const int* det_id,
+                            const int* gt_obj, const int* gt_points, const int* seq_start, int S, int B, int M, int C,
+                            int K, int n_obj, int cap, int* last_id, long long* counts, double* dist, void* workspace,
+                            cudaStream_t stream) {
+  const MotArgs a{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, e_iou, det_pass, det_id, gt_obj,
+                  gt_points, seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, counts, dist, workspace};
+  int rc = check_mot_args(a);
+  if (rc) return rc;
+  const long long rows = (long long)S * C * K;
+  if (rows == 0) return PNX_OK;
+  PNX_CHECK_ARG(workspace, "workspace");
+  if (n_obj > 0) PNX_CUDA(cudaMemsetAsync(last_id, 0xff, (size_t)K * n_obj * sizeof(int), stream));
+  eval_mot_kernel<<<(unsigned)rows, 32, 0, stream>>>(a);
+  PNX_CHECK_LAUNCH();
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_mot_host(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                                 const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box,
+                                 const float* e_iou, long long n_det, const int* det_pass, const int* det_id,
+                                 const int* gt_obj, const int* gt_points, const int* seq_start, int S, int B, int M,
+                                 int C, int K, int n_obj, int cap, int* last_id, long long* counts, double* dist) {
+  const MotArgs a{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, e_iou, det_pass, det_id, gt_obj,
+                  gt_points, seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, counts, dist, nullptr};
+  int rc = check_mot_args(a);
+  if (rc) return rc;
+  for (long long i = 0; i < (long long)K * n_obj; ++i) last_id[i] = -1;
+  char* ws = new char[mot_row_bytes(M, cap)];
+  int scal[2];
+  const CompMem m = workspace_mem(ws, cap, 0, scal);
+  for (long long row = 0; row < (long long)S * C * K; ++row)
+    mot_row(HostGroup{}, a, (int)row, m, (int*)(ws + mot_comp_bytes(cap)));
+  delete[] ws;
   return PNX_OK;
 }

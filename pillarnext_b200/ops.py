@@ -1396,3 +1396,123 @@ def eval_match_center_host(det_boxes, order, seg_start, seg_count, gt_boxes, gt_
     check(lib().pnx_eval_match_center_host(_hp(db), D, _hp(od), _hp(ss), _hp(sc), _hp(gb), _hp(gc), B, M, C, _hp(th), T,
                                            _hp(match)))
     return match
+
+
+# --------------------------------------------------------------------------------- tracking
+def _track_operands(boxes, scores, order, seg_start, seg_count, poses, times, seq_start, max_dist, host=False):
+    D, F, C = len(boxes), len(poses), len(max_dist)
+    f32, i32, i64 = torch.float32, torch.int32, torch.int64
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (boxes, f32, (D, 9), "boxes"), (scores, f32, (D,), "scores"), (order, i64, (D,), "order"),
+        (seg_start, i32, (F * C,), "seg_start"), (seg_count, i32, (F * C,), "seg_count"),
+        (poses, torch.float64, (F, 4, 4), "poses"), (times, i64, (F,), "times"),
+        (seq_start, i32, (len(seq_start),), "seq_start"), (max_dist, f32, (C,), "max_dist"))]
+
+
+def _track_status(status, C):
+    if status:
+        raise ValueError("sequence %d, class %d: more than %d live tracks at once" %
+                         ((status - 1) // C, (status - 1) % C, lib().pnx_track_max_tracks()))
+
+
+def track_greedy(boxes, scores, order, seg_start, seg_count, poses, times, seq_start, max_dist, max_age, min_score):
+    """The greedy velocity tracker (pnx_track_greedy, include/pnx.h), all CUDA: boxes [D, 9] fp32, scores [D] fp32,
+    order [D] int64 (by segment f C + c, then descending score), seg_start / seg_count [F C] int32, poses [F, 4, 4]
+    fp64, times [F] int64 microseconds, seq_start [S + 1] int32, max_dist [C] fp32 -> track_id [D] int64 (-1 below
+    min_score).  Reads the largest segment and one status word back: raises ValueError when a (sequence, class)
+    exceeds the track capacity."""
+    ops_ = _track_operands(boxes, scores, order, seg_start, seg_count, poses, times, seq_start, max_dist)
+    D, F, C, S = len(ops_[0]), len(ops_[5]), len(ops_[8]), len(ops_[7]) - 1
+    dev = ops_[0].device
+    per_row = torch.zeros(S * C + 1, dtype=torch.int64, device=dev)
+    if D:
+        seq_of_frame = torch.repeat_interleave(torch.arange(S, device=dev), (ops_[7][1:] - ops_[7][:-1]).long(),
+                                               output_size=F)
+        row_of_seg = (seq_of_frame[:, None] * C + torch.arange(C, device=dev)).view(-1)
+        per_row.index_add_(0, row_of_seg + 1, ops_[4].long())
+    row_det_start = torch.cumsum(per_row, 0)[:-1].contiguous()
+    local_id, scratch = (torch.empty(max(D, 1), dtype=torch.int32, device=dev) for _ in range(2))
+    births = torch.empty(max(S * C, 1), dtype=torch.int32, device=dev)
+    track_id = torch.empty(D, dtype=torch.int64, device=dev)
+    status = torch.empty(1, dtype=torch.int32, device=dev)
+    # slots enough for every track that can be live (matched or born in the last max_age + 1 frames, plus this
+    # frame's births), at most the library's capacity: a smaller table keeps more warps per SM
+    cap = min(lib().pnx_track_max_tracks(), (int(max_age) + 2) * max(1, int(ops_[4].max()) if F * C else 1))
+    _count(2)
+    check(lib().pnx_track_greedy(ptr(ops_[0]), ptr(ops_[1]), D, *[ptr(t) for t in ops_[2:8]], S, F, C, ptr(ops_[8]),
+                                 int(max_age), float(min_score), cap, ptr(row_det_start), ptr(local_id), ptr(births),
+                                 ptr(scratch), ptr(track_id), ptr(status), stream()))
+    _track_status(int(status.item()), C)
+    return track_id
+
+
+def track_greedy_host(boxes, scores, order, seg_start, seg_count, poses, times, seq_start, max_dist, max_age, min_score):
+    """Host twin of track_greedy (pnx_track_greedy_host): the same operands as numpy arrays -> track_id [D] int64."""
+    ops_ = _track_operands(boxes, scores, order, seg_start, seg_count, poses, times, seq_start, max_dist, host=True)
+    D, F, C, S = len(ops_[0]), len(ops_[5]), len(ops_[8]), len(ops_[7]) - 1
+    track_id, status = np.zeros(D, np.int64), np.zeros(1, np.int32)
+    check(lib().pnx_track_greedy_host(_hp(ops_[0]), _hp(ops_[1]), D, *[_hp(t) for t in ops_[2:8]], S, F, C,
+                                      _hp(ops_[8]), int(max_age), float(min_score), _hp(track_id), _hp(status)))
+    _track_status(int(status[0]), C)
+    return track_id
+
+
+def _eval_mot_operands(edge_start, e_det, e_box, e_iou, grouped, comp_start, comp_nedge, det_pass, det_id, gt_obj,
+                       gt_points, seq_start, host=False):
+    E, D, BM = len(e_det), len(det_pass), len(gt_obj)
+    i32 = torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (edge_start, i32, (len(edge_start),), "edge_start"), (grouped, i32, (E,), "grouped"),
+        (comp_start, i32, (E,), "comp_start"), (comp_nedge, i32, (E,), "comp_nedge"), (e_det, i32, (E,), "e_det"),
+        (e_box, i32, (E,), "e_box"), (e_iou, torch.float32, (E,), "e_iou"), (det_pass, i32, (D,), "det_pass"),
+        (det_id, i32, (D,), "det_id"), (gt_obj, i32, (BM,), "gt_obj"), (gt_points, i32, (BM,), "gt_points"),
+        (seq_start, i32, (len(seq_start),), "seq_start"))]
+
+
+def _mot_cap(comp_nedge):
+    """Pairs one row's assignment state must hold: the largest component, at least the one-warp size + 2."""
+    big = int(comp_nedge.max()) if len(comp_nedge) else 0
+    return max(big, lib().pnx_eval_assign_warp_pairs() + 2)
+
+
+def eval_mot(edge_start, e_det, e_box, e_iou, grouped, comp_start, comp_nedge, det_pass, det_id, gt_obj, gt_points,
+             seq_start, M, n_classes, K, n_obj):
+    """CLEAR-MOT frame matching per (sequence, class, cutoff) (pnx_eval_mot, include/pnx.h), all CUDA: the pairs of
+    eval_pairs, the components of eval_components, det_pass / det_id [D] int32, gt_obj / gt_points [B M] int32,
+    seq_start [S + 1] int32 -> (counts [S, C, K, 5] int64, dist [S, C, K, 2] fp64).  One host read (the largest
+    component) sizes the workspace: every (sequence, class, cutoff) row gets 164 B per pair of the largest component
+    anywhere plus 4 B per box slot, so S C K (164 cap + 4 M) bytes in all (Waymo val: 6600 rows, 37 MB at the
+    one-warp minimum of 34 pairs; a crowd component of 2000 pairs would take 2.2 GB)."""
+    ops_ = _eval_mot_operands(edge_start, e_det, e_box, e_iou, grouped, comp_start, comp_nedge, det_pass, det_id,
+                              gt_obj, gt_points, seq_start)
+    st = ops_[0]
+    E, D, S, C, B = len(ops_[4]), len(ops_[7]), len(ops_[11]) - 1, int(n_classes), len(st) // int(n_classes)
+    dev = st.device
+    cap = _mot_cap(ops_[3])
+    count = _edge_count(st, E)
+    counts = torch.empty((S, C, int(K), 5), dtype=torch.int64, device=dev)
+    dist = torch.empty((S, C, int(K), 2), dtype=torch.float64, device=dev)
+    last_id = torch.empty(max(1, int(K) * int(n_obj)), dtype=torch.int32, device=dev)
+    ws = torch.empty(max(1, lib().pnx_eval_mot_workspace(S * C * int(K), int(M), cap)), dtype=torch.uint8, device=dev)
+    _count(1)
+    check(lib().pnx_eval_mot(ptr(st), ptr(count), E, *[ptr(t) for t in ops_[1:7]], D,
+                             *[ptr(t) for t in ops_[7:]], S, B, int(M), C, int(K), int(n_obj), cap, ptr(last_id),
+                             ptr(counts), ptr(dist), ptr(ws), stream()))
+    return counts, dist
+
+
+def eval_mot_host(edge_start, e_det, e_box, e_iou, grouped, comp_start, comp_nedge, det_pass, det_id, gt_obj,
+                  gt_points, seq_start, M, n_classes, K, n_obj):
+    """Host twin of eval_mot (pnx_eval_mot_host): numpy in -> (counts [S, C, K, 5] int64, dist [S, C, K, 2] fp64)."""
+    ops_ = _eval_mot_operands(edge_start, e_det, e_box, e_iou, grouped, comp_start, comp_nedge, det_pass, det_id,
+                              gt_obj, gt_points, seq_start, host=True)
+    st = ops_[0]
+    E, D, S, C, B = len(ops_[4]), len(ops_[7]), len(ops_[11]) - 1, int(n_classes), len(st) // int(n_classes)
+    cap = _mot_cap(ops_[3])
+    count = _edge_count(st, E)
+    counts, dist = np.zeros((S, C, int(K), 5), np.int64), np.zeros((S, C, int(K), 2), np.float64)
+    last_id = np.zeros(max(1, int(K) * int(n_obj)), np.int32)
+    check(lib().pnx_eval_mot_host(_hp(st), _hp(count), E, *[_hp(t) for t in ops_[1:7]], D,
+                                  *[_hp(t) for t in ops_[7:]], S, B, int(M), C, int(K), int(n_obj), cap,
+                                  _hp(last_id), _hp(counts), _hp(dist)))
+    return counts, dist

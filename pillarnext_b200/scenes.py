@@ -146,6 +146,31 @@ def make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=0.05, ego_speed=5.0
     return pts[order], T, owner[order]
 
 
+SEQUENCE_STEP_US = 100000           # frames of a sequence are 0.1 s apart
+SEQUENCE_T0_US = 1000000000         # timestamp of every sequence's first frame
+
+
+def sequence_frame(seed, k, cfg, n_points=6000, n_boxes=12, ego_speed=5.0):
+    """Frame k >= 0 of the sequence that starts with make_scene(seed): the scene k * 0.1 s later, with make_sweep's
+    motion run forward (each box at centre + v * 0.1 k, the ego on ego_pose's arc), scanned from the ego's pose then.
+    Returns (points [N, 5] fp32 with time 0, boxes [M, 9] fp32 in frame k's sensor frame -- velocity rotated into it,
+    the order and so the object ids of make_scene's boxes --, names, pose [4, 4] fp64 frame k's sensor -> the first
+    frame's sensor).  Frame 0 is exactly make_scene(seed) with the identity pose."""
+    pts, boxes, names = make_scene(seed, cfg, n_points, n_boxes)
+    if k == 0:
+        return pts, boxes, names, np.eye(4)
+    p, T, _ = make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=-SEQUENCE_STEP_US * 1e-6, ego_speed=ego_speed)
+    p[:, 4] = 0.0
+    lag = k * -SEQUENCE_STEP_US * 1e-6                              # make_sweep's box motion, and the velocity
+    b = boxes.astype(np.float64).copy()
+    b[:, :2] -= b[:, 6:8] * lag
+    R, t = T[:2, :2], T[:2, 3]
+    b[:, :2] = (b[:, :2] - t) @ R
+    b[:, 6:8] = b[:, 6:8] @ R
+    b[:, 8] -= np.arctan2(T[1, 0], T[0, 0])
+    return p, b.astype(np.float32), names, T
+
+
 def sampling_record(sampler, boxes, names, class_names):
     """The `gts` record of one frame: the candidates sampler.sample_all draws for the scene boxes [M, 9] fp32 named
     `names` (none drawn = zero candidates), their classes as indices into class_names, and numpy's (cos, sin) of the
@@ -164,6 +189,9 @@ def sampling_record(sampler, boxes, names, class_names):
     return {"boxes": rec["gt_boxes"], "classes": np.array([class_names.index(n) for n in rec["gt_names"]], np.int32),
             "points": rec["points"], "num_points": rec["num_points"], "trig": rec["trig"],
             "scene_trig": numpy_trig(boxes)}
+
+
+METRICS = ("nuscenes", "waymo", "nds", "waymo_tracking")
 
 
 class SyntheticSceneDataset(torch.utils.data.Dataset):
@@ -186,15 +214,23 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     takes the sweeps into the key frame on the GPU (ops.accumulate_sweeps), dropping the sweep points within
     min_distance of the sensor in x and y (nuScenes' remove_close; 0 = off).  nsweeps = 1 frames are unchanged.
 
+    sequence_length: frames are grouped into sequences of that many frames, 0.1 s apart (sequence_frame: sequence q
+    starts with make_scene(seed0 + q L); its objects keep their ids and move by their velocity labels, the ego follows
+    ego_pose).  Each frame's token is then "seq<seed>-<timestamp_micros>" and ground_truth() carries its sequence,
+    timestamp, pose and the objects' ids.  The default 1 leaves every frame and token as they were.  Sequences do not
+    take sweeps (nsweeps must be 1).
+
     metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map), "waymo" (evaluate_waymo.waymo_metrics,
-    AP / APH at LEVEL_1 and LEVEL_2) or "nds" (evaluate_nuscenes.nuscenes_metrics, the nuScenes detection score with
-    its true-positive errors).  For "waymo" and "nds" ground_truth() also hands over each frame's points.
+    AP / APH at LEVEL_1 and LEVEL_2), "nds" (evaluate_nuscenes.nuscenes_metrics, the nuScenes detection score with
+    its true-positive errors) or "waymo_tracking" (the "waymo" dict plus "tracking": the detections tracked by
+    track.track and scored by evaluate_waymo_tracking.waymo_tracking_metrics).  For every metric but "nuscenes"
+    ground_truth() also hands over each frame's points.
     waymo_matching: for metric "waymo", "greedy" (the default) or "hungarian" (the maximum-IoU matching at score-cutoff
     quantiles with the range breakdown, evaluate_waymo.py)."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
                  augmentation=None, sampler=None, root_path=None, metric="nuscenes", nsweeps=1, drop_frames=0.0,
-                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, waymo_matching="greedy", **_):
+                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, waymo_matching="greedy", sequence_length=1, **_):
         if int(nsweeps) < 1 or not 0.0 <= drop_frames <= 1.0 or min_distance < 0:
             raise ValueError("nsweeps must be >= 1, drop_frames in [0, 1] and min_distance >= 0, got %r, %r, %r"
                              % (nsweeps, drop_frames, min_distance))
@@ -202,8 +238,11 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         self.sweep_interval, self.ego_speed, self.min_distance = float(sweep_interval), float(ego_speed), float(min_distance)
         self.cfg, self.n_frames, self.seed0, self.n_points, self.n_boxes = cfg, int(n_frames), int(seed0), int(n_points), int(n_boxes)
         self.test_mode = test_mode
-        if metric not in ("nuscenes", "waymo", "nds"):
-            raise ValueError("metric must be 'nuscenes', 'waymo' or 'nds', got %r" % (metric,))
+        if metric not in METRICS:
+            raise ValueError("metric must be one of %s, got %r" % (METRICS, metric))
+        self.sequence_length = int(sequence_length)
+        if self.sequence_length < 1 or (self.sequence_length > 1 and self.nsweeps > 1):
+            raise ValueError("sequence_length must be >= 1, and 1 when nsweeps > 1, got %r" % (sequence_length,))
         self.metric = metric
         from .evaluate_waymo import check_matching
         self.waymo_matching = check_matching(waymo_matching)
@@ -221,10 +260,21 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     def __len__(self):
         return self.n_frames
 
+    def _frame(self, i):
+        """(points, boxes, names, token, sequence, timestamp, pose) of frame i."""
+        if self.sequence_length == 1:
+            pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
+            return pts, boxes, names, "scene_%d" % (self.seed0 + i), None, None, None
+        q, k = divmod(i, self.sequence_length)
+        seed = self.seed0 + q * self.sequence_length
+        pts, boxes, names, pose = sequence_frame(seed, k, self.cfg, self.n_points, self.n_boxes, self.ego_speed)
+        ts = SEQUENCE_T0_US + k * SEQUENCE_STEP_US
+        return pts, boxes, names, "seq%d-%d" % (seed, ts), "seq%d" % seed, ts, pose
+
     def __getitem__(self, i):
-        pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
+        pts, boxes, names, token = self._frame(i)[:4]
         cls = np.array([self.class_names.index(n) for n in names], dtype=np.int32)
-        res = {"points": pts, "gt_boxes_raw": boxes, "gt_classes": cls, "token": "scene_%d" % (self.seed0 + i)}
+        res = {"points": pts, "gt_boxes_raw": boxes, "gt_classes": cls, "token": token}
         if self.nsweeps > 1:
             res["sweeps"] = self._sweeps(self.seed0 + i, boxes)
         if self.sampler is not None:
@@ -254,17 +304,24 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     def ground_truth(self):
         gts = {}
         for i in range(self.n_frames):
-            pts, boxes, names = make_scene(self.seed0 + i, self.cfg, self.n_points, self.n_boxes)
-            gts["scene_%d" % (self.seed0 + i)] = {"boxes": boxes, "names": names}
-            if self.metric in ("waymo", "nds"):
-                gts["scene_%d" % (self.seed0 + i)]["points"] = pts
+            pts, boxes, names, token, seq, ts, pose = self._frame(i)
+            gts[token] = {"boxes": boxes, "names": names}
+            if self.metric != "nuscenes":
+                gts[token]["points"] = pts
+            if seq is not None:
+                gts[token].update(ids=[str(j) for j in range(len(names))], sequence=seq, timestamp=ts, pose=pose)
         return gts
 
     def evaluation(self, detections, output_dir=None, testset=False):
         """The hook the reference trainer calls at the end of val_epoch (base.py:48-51, trainer.py:165-184)."""
-        if self.metric == "waymo":
+        if self.metric in ("waymo", "waymo_tracking"):
             from .evaluate_waymo import waymo_metrics
-            return waymo_metrics(self.ground_truth(), detections, self.class_names, matching=self.waymo_matching)
+            gts = self.ground_truth()
+            res = waymo_metrics(gts, detections, self.class_names, matching=self.waymo_matching)
+            if self.metric == "waymo_tracking":
+                from .evaluate_waymo_tracking import track_and_score
+                res["tracking"] = track_and_score(gts, detections, self.class_names)[1]
+            return res
         if self.metric == "nds":
             from .evaluate_nuscenes import nuscenes_metrics
             return nuscenes_metrics(self.ground_truth(), detections, self.class_names)
