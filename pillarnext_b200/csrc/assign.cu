@@ -51,10 +51,10 @@ __device__ double gaussian_radius(double height, double width, double min_overla
 
 __global__ void __launch_bounds__(kAssignThreads) assign_kernel(AssignParams p) {
   __shared__ int s_scan[kAssignThreads / 32];
-  __shared__ int s_base;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_base = 0;
-  __syncthreads();
+  // running slot base of the chunk: every thread keeps it in a register and adds all of s_scan once the barrier has
+  // published it, so no thread writes shared state that another warp of the same barrier interval still reads
+  int base = 0;
   for (int k0 = 0; k0 < p.N; k0 += kAssignThreads) {
     const int k = k0 + tid;
     bool ok = false;
@@ -81,8 +81,9 @@ __global__ void __launch_bounds__(kAssignThreads) assign_kernel(AssignParams p) 
     const unsigned int bal = __ballot_sync(0xffffffffu, ok);
     if (lane == 0) s_scan[warp] = __popc(bal);
     __syncthreads();
-    int before = s_base + __popc(bal & ((1u << lane) - 1u));
+    int before = base + __popc(bal & ((1u << lane) - 1u));
     for (int w = 0; w < warp; ++w) before += s_scan[w];
+    for (int w = 0; w < kAssignThreads / 32; ++w) base += s_scan[w];
     if (ok && before < p.M) {
       const size_t o = (size_t)b * p.M + before;
       p.cat[o] = cid;
@@ -104,12 +105,7 @@ __global__ void __launch_bounds__(kAssignThreads) assign_kernel(AssignParams p) 
       int4 o = make_int4(ok ? cxi : -1, cyi, radius, cid);
       reinterpret_cast<int4*>(p.obj)[(size_t)b * p.N + k] = o;
     }
-    if (tid == 0) {
-      int tot = 0;
-      for (int w = 0; w < kAssignThreads / 32; ++w) tot += s_scan[w];
-      s_base += tot;
-    }
-    __syncthreads();
+    __syncthreads();  // s_scan is rewritten by the next chunk
   }
 }
 
