@@ -9,7 +9,16 @@ them into the key frame on the GPU (ops.accumulate_sweeps), with the reference's
 
 evaluation() writes the devkit's results JSON, <info name>.json; the boxes go to the global frame through each info's
 ref_from_car and car_from_global matrices (the devkit's pose records are not read).  When the infos carry gt_boxes it
-also returns evaluate_nuscenes.nuscenes_metrics, with the points counted in the key-frame files."""
+also returns evaluate_nuscenes.nuscenes_metrics, with the points counted in the key-frame files.
+
+tracking=True (not a reference argument) also tracks the detections of the nuScenes tracking classes through each
+scene (evaluate_nuscenes_tracking.track_and_score's tracker: track.track with track.NUSCENES_MAX_DIST).  Each token's
+scene_token and integer timestamp (microseconds) come from <root_path>/<version>/sample.json, the devkit's plain-JSON
+sample table (no devkit needed); its pose is the lidar -> global transform of ref_from_car / car_from_global.
+evaluation() then writes the devkit's tracking-results JSON, <info name>_tracking.json (sample_token, translation,
+size, rotation, velocity, tracking_id as a string, tracking_name, tracking_score, and the meta block), and returns the
+tracks under "tracks" (the metrics dict, or {} when there is none).  The infos carry no instance tokens, so the tracks
+are not scored here.  With tracking=False nothing changes."""
 import itertools
 import json
 import os
@@ -20,6 +29,8 @@ import numpy as np
 from det3d.datasets.base import BaseDataset
 from pillarnext_b200.evaluate_nuscenes import (DEFAULT_ATTRIBUTE, MOVING_ATTRIBUTE, MOVING_SPEED, STILL_ATTRIBUTE,
                                                nuscenes_metrics)
+
+META = {"use_camera": False, "use_lidar": True, "use_radar": False, "use_map": False, "use_external": False}
 
 
 def attribute(name, velocity):
@@ -44,16 +55,32 @@ def _quaternion(R):
     return [float(-v if q[0] < 0 else v) for v in q]
 
 
+def lidar_to_global(info):
+    """4x4 lidar -> global of an info: the inverse of ref_from_global = ref_from_car @ car_from_global."""
+    return np.linalg.inv(np.asarray(info["ref_from_car"]) @ np.asarray(info["car_from_global"]))
+
+
+def global_box(b, to_global):
+    """One box (x, y, z, dx, dy, dz, vx, vy, yaw) in fp64 -> the devkit's (translation, size, rotation quaternion,
+    velocity (vx, vy)) in the global frame, and the 3-D global velocity (for the attribute rule)."""
+    yaw = b[8]
+    Rl = np.array([[np.cos(yaw), -np.sin(yaw), 0], [np.sin(yaw), np.cos(yaw), 0], [0, 0, 1]])
+    velocity = to_global[:3, :3] @ np.array([b[6], b[7], 0.0])
+    return ((to_global[:3, :3] @ b[:3] + to_global[:3, 3]).tolist(), [float(b[4]), float(b[3]), float(b[5])],
+            _quaternion(to_global[:3, :3] @ Rl), velocity[:2].tolist()), velocity
+
+
 class NuScenesDataset(BaseDataset):
     def __init__(self, info_path, root_path, nsweeps, sampler=None, loading_pipelines=None, augmentation=None,
                  prepare_label=None, class_names=[], resampling=False, evaluations=None, create_database=False,
-                 use_gt_sampling=True, version="v1.0-trainval"):
+                 use_gt_sampling=True, version="v1.0-trainval", tracking=False):
         super().__init__(root_path, info_path, sampler, loading_pipelines, augmentation, prepare_label, evaluations,
                          create_database, use_gt_sampling=use_gt_sampling)
         self.nsweeps = nsweeps
         assert self.nsweeps > 0, "At least input one sweep please!"
         self._class_names = list(itertools.chain(*[t for t in class_names]))
         self.version = version
+        self.tracking = bool(tracking)
         if resampling:
             self.cbgs()
 
@@ -102,39 +129,75 @@ class NuScenesDataset(BaseDataset):
                                       "names": list(info["gt_names"]), "points": self.read_file(str(info["lidar_path"]))}
         return gts
 
+    def frames(self, tokens):
+        """token -> {"sequence" (scene_token), "timestamp" (int microseconds), "pose" (lidar -> global)} of the infos
+        of `tokens`, from <root_path>/<version>/sample.json."""
+        with open(os.path.join(self._root_path, self.version, "sample.json")) as f:
+            samples = {s["token"]: s for s in json.load(f)}
+        infos = {info["token"]: info for info in self.infos}
+        missing = [t for t in tokens if t not in samples]
+        if missing:
+            raise ValueError("tokens missing from %s/sample.json: %s" % (self.version, missing[:5]))
+        return {t: {"sequence": str(samples[t]["scene_token"]), "timestamp": int(samples[t]["timestamp"]),
+                    "pose": lidar_to_global(infos[t])} for t in tokens}
+
     def evaluation(self, detections, output_dir=None, testset=False):
         infos = {info["token"]: info for info in self.infos}
         results = {}
         for token, det in detections.items():
-            info = infos[token]
-            # lidar -> global: the inverse of ref_from_global = ref_from_car @ car_from_global
-            to_global = np.linalg.inv(np.asarray(info["ref_from_car"]) @ np.asarray(info["car_from_global"]))
+            to_global = lidar_to_global(infos[token])
             boxes = np.asarray(det["box3d_lidar"], np.float64).reshape(-1, 9)
             scores = np.asarray(det["scores"], np.float64).reshape(-1)
             labels = np.asarray(det["label_preds"]).reshape(-1)
             annos = []
             for b, s, l in zip(boxes, scores, labels):
                 name = self._class_names[int(l)]
-                yaw = b[8]
-                Rl = np.array([[np.cos(yaw), -np.sin(yaw), 0], [np.sin(yaw), np.cos(yaw), 0], [0, 0, 1]])
-                velocity = to_global[:3, :3] @ np.array([b[6], b[7], 0.0])
+                (translation, size, rotation, vel), velocity = global_box(b, to_global)
                 annos.append({
                     "sample_token": token,
-                    "translation": (to_global[:3, :3] @ b[:3] + to_global[:3, 3]).tolist(),
-                    "size": [float(b[4]), float(b[3]), float(b[5])],
-                    "rotation": _quaternion(to_global[:3, :3] @ Rl),
-                    "velocity": velocity[:2].tolist(),
+                    "translation": translation,
+                    "size": size,
+                    "rotation": rotation,
+                    "velocity": vel,
                     "detection_name": name,
                     "detection_score": float(s),
                     "attribute_name": attribute(name, velocity),
                 })
             results[token] = annos
-        out = {"results": results, "meta": {"use_camera": False, "use_lidar": True, "use_radar": False,
-                                             "use_map": False, "use_external": False}}
+        out = {"results": results, "meta": dict(META)}
         name = str(self._info_path).split("/")[-1].split(".")[0]
         with open(Path(output_dir) / (name + ".json"), "w") as f:
             json.dump(out, f)
+        tracks = self.write_tracks(detections, Path(output_dir) / (name + "_tracking.json")) if self.tracking else None
         gts = self.ground_truth()
         if testset or not gts:
-            return None
-        return nuscenes_metrics(gts, detections, self._class_names)
+            return None if tracks is None else {"tracks": tracks}
+        res = nuscenes_metrics(gts, detections, self._class_names)
+        if tracks is not None:
+            res["tracks"] = tracks
+        return res
+
+    def write_tracks(self, detections, path, host=False):
+        """Tracks the detections through each scene and writes the devkit's tracking-results JSON to `path` ->
+        token -> the tracks (detections of the tracking classes with "tracking_id").  host=True tracks with the
+        tracker's host twin."""
+        from pillarnext_b200.evaluate_nuscenes_tracking import track_detections
+        frames = self.frames(list(detections))
+        tracks = track_detections(frames, detections, self._class_names, host=host)
+        results = {}
+        for token, d in tracks.items():
+            to_global = frames[token]["pose"]
+            boxes = np.asarray(d["box3d_lidar"], np.float64).reshape(-1, 9)
+            annos = []
+            for b, s, l, i in zip(boxes, np.asarray(d["scores"], np.float64).reshape(-1),
+                                  np.asarray(d["label_preds"]).reshape(-1), np.asarray(d["tracking_id"]).reshape(-1)):
+                if i < 0:
+                    continue
+                (translation, size, rotation, vel), _ = global_box(b, to_global)
+                annos.append({"sample_token": token, "translation": translation, "size": size, "rotation": rotation,
+                              "velocity": vel, "tracking_id": str(int(i)), "tracking_name": self._class_names[int(l)],
+                              "tracking_score": float(s)})
+            results[token] = annos
+        with open(path, "w") as f:
+            json.dump({"results": results, "meta": dict(META)}, f)
+        return tracks

@@ -610,6 +610,45 @@ int pnx_eval_match_center_host(const float* det_boxes, long long n_det, const lo
                                const int* seg_count, const float* gt_boxes, const int* gt_classes, int B, int M, int C,
                                const double* dist_ths, int T, int* match);
 
+/* ------------------------------------------------ nuScenes tracking (pillarnext_b200/evaluate_nuscenes_tracking.py)
+ * pnx_eval_pairs_center: the pairs of every (frame, class) segment whose centre distance (pnx_eval_match_center's
+ *   fp64 arithmetic) is < max_dist, 0 < max_dist <= 2 metres.  Operands as for pnx_eval_match_center (order: by
+ *   segment, then in visit order); outputs laid out as pnx_eval_pairs': edge_start null -> edge_count [B C] only;
+ *   edge_start [B C] -> e_det, e_box = f M + j, e_dist = the distance rounded to fp32, detections in visit order, each
+ *   one's boxes in ascending j.
+ * pnx_eval_mot_center: pnx_eval_mot's frame walk, rows (S, C, K), carry-over and operands (e_dist in place of e_iou),
+ *   with another assignment weight and other counts.  The assignment takes the most pairs, then the smallest sum of
+ *   distances, ties by pnx_eval_assign's rule: it maximises 2^40 - round(e_dist 2^26) per pair, and as a component
+ *   has at most M <= 2^12 matches of at most 2^27 each, one more match outweighs any distance sum.  gt_prev [B M]
+ *   int32 = the frame of the same object's previous box (-1 for its first, or no object).  Outputs counts [S, C, K, 3]
+ *   int64 = matches, identity switches (a match whose id differs from the object's last matched id), fragmentations
+ *   (a match of an object that was matched before and has a box in a frame after that match); dist [S, C, K] fp64 =
+ *   the sum of the matches' e_dist in match order; matched [n_det] uint8 (null, or K = 1 only) = 1 for each matched
+ *   detection, else 0.  last_id, last_frame [K, n_obj] int32 scratch.  cap as for pnx_eval_mot; workspace =
+ *   pnx_eval_mot_workspace(S C K, M, cap) bytes (the same row layout).
+ * Both run on `stream` with no host sync; the _host twins take HOST memory and no workspace, and equal them bit for
+ * bit. */
+int pnx_eval_pairs_center(const float* det_boxes, long long n_det, const long long* order, const int* seg_start,
+                          const int* seg_count, const float* gt_boxes, const int* gt_classes, int B, int M, int C,
+                          double max_dist, const int* edge_start, int* edge_count, int* e_det, int* e_box,
+                          float* e_dist, cudaStream_t stream);
+int pnx_eval_pairs_center_host(const float* det_boxes, long long n_det, const long long* order, const int* seg_start,
+                               const int* seg_count, const float* gt_boxes, const int* gt_classes, int B, int M, int C,
+                               double max_dist, const int* edge_start, int* edge_count, int* e_det, int* e_box,
+                               float* e_dist);
+int pnx_eval_mot_center(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                        const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box,
+                        const float* e_dist, long long n_det, const int* det_pass, const int* det_id, const int* gt_obj,
+                        const int* gt_prev, const int* seq_start, int S, int B, int M, int C, int K, int n_obj, int cap,
+                        int* last_id, int* last_frame, long long* counts, double* dist, unsigned char* matched,
+                        void* workspace, cudaStream_t stream);
+int pnx_eval_mot_center_host(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                             const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box,
+                             const float* e_dist, long long n_det, const int* det_pass, const int* det_id,
+                             const int* gt_obj, const int* gt_prev, const int* seq_start, int S, int B, int M, int C,
+                             int K, int n_obj, int cap, int* last_id, int* last_frame, long long* counts, double* dist,
+                             unsigned char* matched);
+
 #ifdef __cplusplus
 }
 #endif

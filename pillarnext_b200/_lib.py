@@ -125,6 +125,11 @@ _SIGS = {
     # nuScenes detection score: the centre-distance match, per threshold
     "pnx_eval_match_center": [P, L, P, P, P, P, P, I, I, I, P, I, P, P],
     "pnx_eval_match_center_host": [P, L, P, P, P, P, P, I, I, I, P, I, P],
+    # nuScenes tracking: centre-distance pairs and the frame matching of evaluate_nuscenes_tracking
+    "pnx_eval_pairs_center": [P, L, P, P, P, P, P, I, I, I, ctypes.c_double, P, P, P, P, P, P],
+    "pnx_eval_pairs_center_host": [P, L, P, P, P, P, P, I, I, I, ctypes.c_double, P, P, P, P, P],
+    "pnx_eval_mot_center": [P, P, L, P, P, P, P, P, P, L, P, P, P, P, P, I, I, I, I, I, I, I, P, P, P, P, P, P, P],
+    "pnx_eval_mot_center_host": [P, P, L, P, P, P, P, P, P, L, P, P, P, P, P, I, I, I, I, I, I, I, P, P, P, P, P],
 }
 _RESTYPE = {"pnx_last_error": ctypes.c_char_p, "pnx_voxelize_bitmap_words": ctypes.c_size_t,
             "pnx_bn_bwd_reduce_split_scratch": ctypes.c_longlong, "pnx_gt_sample_workspace": ctypes.c_longlong,

@@ -34,6 +34,12 @@
 //                          over the pairs left active, its state in the row's slice of a global workspace, and the
 //                          leader counts matches, mismatches and sum(1 - IoU) per level.  The host twin runs the same
 //                          template one row at a time.
+//   pnx_eval_pairs_center  nuScenes tracking's pairs (evaluate_nuscenes_tracking.py), laid out like pnx_eval_pairs: every
+//                          pair with the fp64 centre distance of pnx_eval_match_center < max_dist, written as fp32.
+//   pnx_eval_mot_center    the same frame walk as pnx_eval_mot (mot_row, one warp per (scene, class, cutoff)) with
+//                          another counting rule: the assignment takes the most pairs, then the smallest distance sum,
+//                          and the leader counts matches, identity switches, fragmentations and the distance sum, and
+//                          optionally flags each matched detection.
 // The IoU is the reference's boxes_iou3d_gpu arithmetic (box_geom.cuh det_aligned_iou3d_t) with
 // each box's (cos, sin) of the yaw supplied by the caller, so the kernels, their host twins and the CPU oracle see the
 // same trigonometry.  This file is compiled with -fmad=false (pillarnext_b200/build.py): no multiply-add is
@@ -638,10 +644,11 @@ __host__ __device__ void lex_assign(const G& g, const CompMem& m, int n_d, int n
 }
 
 // Loads the component of pairs ge[0 .. n_e): rows (its detections in visit order), columns (its boxes in ascending
-// index), edge weights and which edges are active (active(e, det, box)).  Returns (n_d, n_g) through m.scal.
-template <class G, class Active>
+// index), edge weights (weight(e), fixed point, maximised) and which edges are active (active(e, det, box)).  Returns
+// (n_d, n_g) through m.scal.
+template <class G, class Weight, class Active>
 __host__ __device__ void load_edges(const G& g, const int* ge, int n_e, const int* e_det, const int* e_box,
-                                    const float* e_iou, const CompMem& m, const Active& active) {
+                                    const Weight& weight, const CompMem& m, const Active& active) {
   for (int l = g.tid(); l < n_e; l += g.size()) {
     const int k = e_box[ge[l]];
     bool first = true;
@@ -655,7 +662,7 @@ __host__ __device__ void load_edges(const G& g, const int* ge, int n_e, const in
     for (int q = 0; q < n_e; ++q) c += m.used[q] && e_box[ge[q]] < k;
     m.col[l] = c;
     if (m.used[l]) m.col_box[c] = k;
-    m.w[l] = (long long)((double)e_iou[e] * kFix);
+    m.w[l] = weight(e);
     m.act[l] = active(e, det, k);
   }
   if (g.leader()) {
@@ -671,6 +678,12 @@ __host__ __device__ void load_edges(const G& g, const int* ge, int n_e, const in
   g.sync();
 }
 
+// The IoU of pair e in 40-bit fixed point: exact for every fp32 IoU >= 2^-17, so the sums compare as the IoU sums do.
+struct IouWeight {
+  const float* e_iou;
+  __host__ __device__ long long operator()(int e) const { return (long long)((double)e_iou[e] * kFix); }
+};
+
 // The detection-metric rule: the detection passes cutoff kc and, in mode 1, lies in the box's range.
 struct CutoffRange {
   const AssignArgs& a;
@@ -683,7 +696,7 @@ struct CutoffRange {
 // Loads component `root` for (mode, cutoff kc).
 template <class G>
 __host__ __device__ void load_component(const G& g, const AssignArgs& a, int root, const CompMem& m, int mode, int kc) {
-  load_edges(g, a.grouped + a.comp_start[root], a.comp_nedge[root], a.e_det, a.e_box, a.e_iou, m,
+  load_edges(g, a.grouped + a.comp_start[root], a.comp_nedge[root], a.e_det, a.e_box, IouWeight{a.e_iou}, m,
              CutoffRange{a, mode, kc});
 }
 
@@ -755,26 +768,31 @@ int check_assign_args(const AssignArgs& a) {
 }
 
 // ---------------------------------------------------------------- CLEAR-MOT frame matching (evaluate_waymo_tracking.py)
-struct MotArgs {
-  const int* edge_start;      // [B C] first pair of each segment (pnx_eval_pairs)
+// The inputs of the frame walk both tracking metrics share.
+struct MotWalk {
+  const int* edge_start;      // [B C] first pair of each segment (pnx_eval_pairs / pnx_eval_pairs_center)
   const int* edge_count;      // [B C]
   const int* grouped;         // [E] components of pnx_eval_components
   const int* comp_start;      // [E]
   const int* comp_nedge;      // [E]
   const int* e_det;           // [E]
   const int* e_box;           // [E] f M + j
-  const float* e_iou;         // [E]
   const int* det_pass;        // [D] number of score cutoffs the detection passes
   const int* det_id;          // [D] tracking id >= 0
   const int* gt_obj;          // [B M] object index in [0, n_obj), -1 = none
-  const int* gt_points;       // [B M] point count (difficulty level)
   const int* seq_start;       // [S + 1] the frames of sequence s are [seq_start[s], seq_start[s + 1])
   int S, B, M, C, K, n_obj, cap;
   long long E, D;
   int* last_id;               // [K, n_obj] the tracking id of each object's last match, -1 = none yet
+  void* workspace;            // [S C K] x mot_row_bytes(M, cap)
+};
+
+struct MotArgs {
+  MotWalk w;
+  const float* e_iou;         // [E]
+  const int* gt_points;       // [B M] point count (difficulty level)
   long long* counts;          // [S, C, K, 5] matches; L1 matches, L1 mismatches; L2 matches, L2 mismatches
   double* dist;               // [S, C, K, 2] sum of 1 - IoU over the L1 / L2 matches
-  void* workspace;            // [S C K] x mot_row_bytes(M, cap)
 };
 
 constexpr int kMotCounts = 5;
@@ -788,7 +806,7 @@ __host__ __device__ inline long long mot_row_bytes(int M, int cap) {
 // Pairs the assignment may use at cutoff kc: the detection passes it, and neither the detection nor the box was kept
 // by the carry-over (kept[j] = the detection holding box j, -1 = none; a detection's pairs are consecutive in [e0, e1)).
 struct MotActive {
-  const MotArgs& a;
+  const MotWalk& a;
   const int* kept;
   int kc, e0, e1;
   __host__ __device__ bool operator()(int e, int det, int k) const {
@@ -801,27 +819,44 @@ struct MotActive {
   }
 };
 
-// One match (detection det, box kb = f M + j, fp32 IoU): the counts of the levels the box belongs to, a mismatch when
-// the object's previous match carried another id, and the object's last id.  n and d as MotArgs::counts / dist.
-__host__ __device__ inline void mot_count(const MotArgs& a, int* last, int det, int kb, float iou, long long* n,
-                                          double* d) {
-  const int o = a.gt_obj[kb], id = a.det_id[det], pts = a.gt_points[kb];
+// The Waymo rule (Rule of mot_row): the maximum-IoU assignment, and per match of (detection det, box kb, pair e) the
+// counts of the levels the box belongs to and sum(1 - IoU).
+struct LevelCounts {
+  const MotArgs& a;
+  IouWeight weight;
+  long long n[kMotCounts] = {0, 0, 0, 0, 0};
+  double d[2] = {0.0, 0.0};
+  __host__ __device__ explicit LevelCounts(const MotArgs& args) : a(args), weight{args.e_iou} {}
+  __host__ __device__ void match(int, int, int, int kb, int e, int, bool mism) {
+    const int pts = a.gt_points[kb];
+    const double miss_iou = 1.0 - (double)a.e_iou[e];
+    ++n[0];
+    if (pts > 5) { ++n[1]; n[2] += mism; d[0] += miss_iou; }
+    if (pts >= 1) { ++n[3]; n[4] += mism; d[1] += miss_iou; }
+  }
+  __host__ __device__ void finish(int row) const {
+    for (int q = 0; q < kMotCounts; ++q) a.counts[(long long)row * kMotCounts + q] = n[q];
+    a.dist[2 * (long long)row] = d[0];
+    a.dist[2 * (long long)row + 1] = d[1];
+  }
+};
+
+// One match: a mismatch when the object's previous match carried another id, the rule's counts, the object's last id.
+template <class Rule>
+__host__ __device__ inline void mot_match(const MotWalk& a, int* last, Rule& r, int kc, int f, int det, int kb, int e) {
+  const int o = a.gt_obj[kb], id = a.det_id[det];
   const bool mism = o >= 0 && last[o] >= 0 && last[o] != id;
+  r.match(kc, f, det, kb, e, o, mism);
   if (o >= 0) last[o] = id;
-  const double miss_iou = 1.0 - (double)iou;
-  ++n[0];
-  if (pts > 5) { ++n[1]; n[2] += mism; d[0] += miss_iou; }
-  if (pts >= 1) { ++n[3]; n[4] += mism; d[1] += miss_iou; }
 }
 
 // One (sequence, class, cutoff) row, frames in order: the carry-over (leader, pairs in order), then every component of
-// the frame's pairs solved by the tie-ruled maximum-IoU assignment over the pairs left active.  Counts on the leader.
-template <class G>
-__host__ __device__ void mot_row(const G& g, const MotArgs& a, int row, const CompMem& m, int* kept) {
+// the frame's pairs solved by the tie-ruled assignment maximising r.weight over the pairs left active.  The rule counts
+// the matches on the leader and writes the row in r.finish.
+template <class G, class Rule>
+__host__ __device__ void mot_row(const G& g, const MotWalk& a, int row, const CompMem& m, int* kept, Rule& r) {
   const int s = row / (a.C * a.K), c = (row / a.K) % a.C, kc = row % a.K;
   int* last = a.last_id + (long long)kc * a.n_obj;
-  long long n[kMotCounts] = {0, 0, 0, 0, 0};
-  double d[2] = {0.0, 0.0};
   for (int f = a.seq_start[s]; f < a.seq_start[s + 1]; ++f) {
     const int seg = f * a.C + c;
     const int e0 = a.edge_start[seg], e1 = e0 + a.edge_count[seg];
@@ -837,16 +872,16 @@ __host__ __device__ void mot_row(const G& g, const MotArgs& a, int row, const Co
         if (o < 0 || last[o] != a.det_id[det]) continue;
         kept[j] = det;
         det_kept = true;
-        mot_count(a, last, det, kb, a.e_iou[e], n, d);
+        mot_match(a, last, r, kc, f, det, kb, e);
       }
     }
     g.sync();
-    for (int r = e0; r < e1; ++r) {
-      if (a.comp_start[r] < 0) continue;                       // not a component's first pair
-      const int* ge = a.grouped + a.comp_start[r];
-      load_edges(g, ge, a.comp_nedge[r], a.e_det, a.e_box, a.e_iou, m, MotActive{a, kept, kc, e0, e1});
+    for (int q = e0; q < e1; ++q) {
+      if (a.comp_start[q] < 0) continue;                       // not a component's first pair
+      const int* ge = a.grouped + a.comp_start[q];
+      load_edges(g, ge, a.comp_nedge[q], a.e_det, a.e_box, r.weight, m, MotActive{a, kept, kc, e0, e1});
       bool any = false;
-      for (int l = 0; l < a.comp_nedge[r]; ++l) any |= m.act[l] != 0;
+      for (int l = 0; l < a.comp_nedge[q]; ++l) any |= m.act[l] != 0;
       if (!any) continue;
       const int n_d = m.scal[0], n_g = m.scal[1];
       lex_assign(g, m, n_d, n_g);
@@ -855,36 +890,207 @@ __host__ __device__ void mot_row(const G& g, const MotArgs& a, int row, const Co
           const int fx = m.fixed[i];
           if (fx > n_g) continue;
           for (int l = m.row_start[i - 1]; l < m.row_start[i]; ++l)
-            if (m.col[l] == fx - 1) { mot_count(a, last, m.row_det[i - 1], a.e_box[ge[l]], a.e_iou[ge[l]], n, d); break; }
+            if (m.col[l] == fx - 1) { mot_match(a, last, r, kc, f, m.row_det[i - 1], a.e_box[ge[l]], ge[l]); break; }
         }
       g.sync();
     }
   }
-  if (g.leader()) {
-    for (int q = 0; q < kMotCounts; ++q) a.counts[(long long)row * kMotCounts + q] = n[q];
-    a.dist[2 * (long long)row] = d[0];
-    a.dist[2 * (long long)row + 1] = d[1];
-  }
+  if (g.leader()) r.finish(row);
 }
 
 // One warp per (sequence, class, cutoff) row, its state in its slice of the workspace.
-__global__ void __launch_bounds__(32) eval_mot_kernel(MotArgs a) {
+template <class Args, class Rule>
+__global__ void __launch_bounds__(32) eval_mot_kernel(Args a) {
   __shared__ int scal[2];
-  char* base = (char*)a.workspace + (long long)blockIdx.x * mot_row_bytes(a.M, a.cap);
-  const CompMem m = workspace_mem(base, a.cap, 0, scal);
-  mot_row(DevGroup<32>{nullptr, nullptr}, a, blockIdx.x, m, (int*)(base + mot_comp_bytes(a.cap)));
+  const MotWalk& w = a.w;
+  char* base = (char*)w.workspace + (long long)blockIdx.x * mot_row_bytes(w.M, w.cap);
+  const CompMem m = workspace_mem(base, w.cap, 0, scal);
+  Rule r(a);
+  mot_row(DevGroup<32>{nullptr, nullptr}, w, blockIdx.x, m, (int*)(base + mot_comp_bytes(w.cap)), r);
 }
 
-int check_mot_args(const MotArgs& a) {
+// The host twin of eval_mot_kernel: every row in turn through one row's workspace.
+template <class Args, class Rule>
+void host_mot(const Args& a) {
+  const MotWalk& w = a.w;
+  for (long long i = 0; i < (long long)w.K * w.n_obj; ++i) w.last_id[i] = -1;
+  char* ws = new char[mot_row_bytes(w.M, w.cap)];
+  int scal[2];
+  const CompMem m = workspace_mem(ws, w.cap, 0, scal);
+  for (long long row = 0; row < (long long)w.S * w.C * w.K; ++row) {
+    Rule r(a);
+    mot_row(HostGroup{}, w, (int)row, m, (int*)(ws + mot_comp_bytes(w.cap)), r);
+  }
+  delete[] ws;
+}
+
+int check_mot_walk(const MotWalk& a) {
   PNX_CHECK_ARG(a.S >= 0 && a.B >= 0 && a.C >= 1 && a.K >= 1 && a.n_obj >= 0, "S / B / C / K / n_obj");
   PNX_CHECK_ARG(a.M >= 1 && a.M <= kMaxBoxesPerFrame, "1 to 4096 boxes per frame");
   PNX_CHECK_ARG((long long)a.S * a.C * a.K < (1LL << 31) && (long long)a.B * a.C < (1LL << 31), "too many rows");
   PNX_CHECK_ARG(a.cap >= kSmallEdges + 2, "cap >= pnx_eval_assign_warp_pairs() + 2");
   PNX_CHECK_ARG(a.E >= 0 && a.E < (1LL << 30) && a.D >= 0 && a.D < (1LL << 31), "number of pairs / detections");
   PNX_CHECK_ARG(a.seq_start && (a.B == 0 || (a.edge_start && a.edge_count)), "segment pointers");
-  PNX_CHECK_ARG(a.E == 0 || (a.grouped && a.comp_start && a.comp_nedge && a.e_det && a.e_box && a.e_iou &&
-                              a.det_pass && a.det_id && a.gt_obj && a.gt_points), "pair pointers");
-  PNX_CHECK_ARG(a.S == 0 || (a.last_id && a.counts && a.dist), "output pointers");
+  PNX_CHECK_ARG(a.E == 0 || (a.grouped && a.comp_start && a.comp_nedge && a.e_det && a.e_box && a.det_pass &&
+                              a.det_id && a.gt_obj), "pair pointers");
+  PNX_CHECK_ARG(a.S == 0 || a.last_id, "last_id");
+  return PNX_OK;
+}
+
+int check_mot_args(const MotArgs& a) {
+  int rc = check_mot_walk(a.w);
+  if (rc) return rc;
+  PNX_CHECK_ARG(a.w.E == 0 || (a.e_iou && a.gt_points), "pair pointers");
+  PNX_CHECK_ARG(a.w.S == 0 || (a.counts && a.dist), "output pointers");
+  return PNX_OK;
+}
+
+// ---------------------------------------------------------------- nuScenes tracking (evaluate_nuscenes_tracking.py)
+// Cardinality first, then the smallest distance sum, in one maximised integer weight per pair: 2^40 - dq with dq =
+// round(d 2^26) of the fp32 distance d <= 2^1 (so dq <= 2^27).  A component's matches are at most its boxes, M <= 2^12,
+// so the dq of any assignment sum to at most 2^39 < 2^40: one more match always outweighs every distance difference.
+constexpr long long kMatchUnit = 1LL << 40;
+constexpr double kDistFix = 67108864.0;      // 2^26: d 2^26 is exact in fp64, + 0.5 rounds half up
+constexpr int kCenterCounts = 3;
+
+struct CenterWeight {
+  const float* e_dist;
+  __host__ __device__ long long operator()(int e) const {
+    return kMatchUnit - (long long)((double)e_dist[e] * kDistFix + 0.5);
+  }
+};
+
+struct CenterMotArgs {
+  MotWalk w;
+  const float* e_dist;        // [E] fp32 centre distance
+  const int* gt_prev;         // [B M] the frame of the object's previous box, -1 = none (first box, or no object)
+  int* last_frame;            // [K, n_obj] the frame of each object's last match, -1 = none yet
+  long long* counts;          // [S, C, K, 3] matches, identity switches, fragmentations
+  double* dist;               // [S, C, K] sum of the matches' fp32 distances
+  unsigned char* matched;     // [D] or null: 1 for each matched detection (K = 1 only)
+};
+
+// The nuScenes rule (Rule of mot_row): the cardinality-first minimum-distance assignment; per match the count, the
+// identity switch, a fragmentation when the object was matched before and has a box after that match, and sum(d).
+struct CenterCounts {
+  const CenterMotArgs& a;
+  CenterWeight weight;
+  long long n[kCenterCounts] = {0, 0, 0};
+  double d = 0.0;
+  __host__ __device__ explicit CenterCounts(const CenterMotArgs& args) : a(args), weight{args.e_dist} {}
+  __host__ __device__ void match(int kc, int f, int det, int kb, int e, int o, bool mism) {
+    ++n[0];
+    n[1] += mism;
+    if (o >= 0) {
+      int* lf = a.last_frame + (long long)kc * a.w.n_obj + o;
+      n[2] += *lf >= 0 && a.gt_prev[kb] > *lf;
+      *lf = f;
+    }
+    d += (double)a.e_dist[e];
+    if (a.matched) a.matched[det] = 1;
+  }
+  __host__ __device__ void finish(int row) const {
+    for (int q = 0; q < kCenterCounts; ++q) a.counts[(long long)row * kCenterCounts + q] = n[q];
+    a.dist[row] = d;
+  }
+};
+
+int check_center_mot_args(const CenterMotArgs& a) {
+  int rc = check_mot_walk(a.w);
+  if (rc) return rc;
+  PNX_CHECK_ARG(a.w.E == 0 || (a.e_dist && a.gt_prev), "pair pointers");
+  PNX_CHECK_ARG(a.w.S == 0 || (a.last_frame && a.counts && a.dist), "output pointers");
+  PNX_CHECK_ARG(!a.matched || a.w.K == 1, "matched flags need K = 1");
+  return PNX_OK;
+}
+
+struct CenterPairArgs {
+  const float* det_boxes;     // [D, 9]
+  const long long* order;     // [D] detection indices, sorted by segment, then in visit order
+  const int* seg_start;       // [B C]
+  const int* seg_count;       // [B C]
+  const float* gt_boxes;      // [B, M, 9]
+  const int* gt_classes;      // [B, M], -1 = padding or filtered out
+  int B, M, C;
+  double max_dist;            // a pair needs centre distance < max_dist
+  long long D;
+  const int* edge_start;      // [B C] or null: count only
+  int* edge_count;            // [B C]
+  int* e_det;                 // [E] detection index
+  int* e_box;                 // [E] f M + j
+  float* e_dist;              // [E] the fp64 distance rounded to fp32
+};
+
+// One warp per (frame, class) segment: every pair with centre distance < max_dist, laid out as eval_pairs_kernel's.
+__global__ void __launch_bounds__(32) eval_pairs_center_kernel(CenterPairArgs p) {
+  extern __shared__ float smem[];
+  const int s = blockIdx.x, lane = threadIdx.x;
+  const int f = s / p.C, c = s - f * p.C;
+  float* xy = smem;                                           // [M, 2] box centres
+  int* idx = (int*)(xy + 2 * (size_t)p.M);                    // [M] box index within the frame
+  const int G = warp_class_boxes(p.gt_classes + (long long)f * p.M, p.M, c, lane, idx);
+  __syncwarp();
+  for (int q = lane; q < G; q += 32) {
+    const float* g = p.gt_boxes + ((long long)f * p.M + idx[q]) * 9;
+    xy[2 * q] = g[0];
+    xy[2 * q + 1] = g[1];
+  }
+  __syncwarp();
+  const int n = p.seg_count[s], base = p.seg_start[s];
+  int cursor = p.edge_start ? p.edge_start[s] : 0;
+  for (int t = 0; t < n; ++t) {
+    const long long di = p.order[base + t];
+    const float* d = p.det_boxes + di * 9;
+    for (int q0 = 0; q0 < G; q0 += 32) {
+      const int q = q0 + lane;
+      const double v = q < G ? center_distance(d, xy + 2 * q) : INFINITY;
+      const bool hit = v < p.max_dist;
+      const unsigned bal = __ballot_sync(0xffffffffu, hit);
+      if (hit && p.edge_start) {
+        const int e = cursor + __popc(bal & ((1u << lane) - 1u));
+        p.e_det[e] = (int)di;
+        p.e_box[e] = f * p.M + idx[q];
+        p.e_dist[e] = (float)v;
+      }
+      cursor += __popc(bal);
+    }
+  }
+  if (lane == 0 && !p.edge_start) p.edge_count[s] = cursor;
+}
+
+void host_pairs_center(const CenterPairArgs& p) {
+  int* idx = new int[p.M > 0 ? p.M : 1];
+  for (long long s = 0; s < (long long)p.B * p.C; ++s) {
+    const int f = (int)(s / p.C), c = (int)(s % p.C);
+    const int G = host_class_boxes(p.gt_classes + (long long)f * p.M, p.M, c, idx);
+    int cursor = p.edge_start ? p.edge_start[s] : 0;
+    for (int t = 0; t < p.seg_count[s]; ++t) {
+      const long long di = p.order[p.seg_start[s] + t];
+      for (int q = 0; q < G; ++q) {
+        const double v = center_distance(p.det_boxes + di * 9, p.gt_boxes + ((long long)f * p.M + idx[q]) * 9);
+        if (!(v < p.max_dist)) continue;
+        if (p.edge_start) {
+          p.e_det[cursor] = (int)di;
+          p.e_box[cursor] = f * p.M + idx[q];
+          p.e_dist[cursor] = (float)v;
+        }
+        ++cursor;
+      }
+    }
+    if (!p.edge_start) p.edge_count[s] = cursor;
+  }
+  delete[] idx;
+}
+
+int check_pairs_center_args(const CenterPairArgs& p) {
+  PNX_CHECK_ARG(p.D >= 0 && p.D < (1LL << 31), "number of detections");
+  PNX_CHECK_ARG(p.B >= 0 && p.C >= 1 && p.M >= 0 && p.M <= kMaxBoxesPerFrame, "B / C / at most 4096 boxes per frame");
+  PNX_CHECK_ARG((long long)p.B * p.C < (1LL << 31), "too many segments");
+  PNX_CHECK_ARG(p.max_dist > 0.0 && p.max_dist <= 2.0, "max_dist in (0, 2] metres");
+  PNX_CHECK_ARG(p.D == 0 || (p.det_boxes && p.order), "detection pointers");
+  PNX_CHECK_ARG((long long)p.B * p.M == 0 || (p.gt_boxes && p.gt_classes), "ground-truth pointers");
+  PNX_CHECK_ARG(p.B == 0 || (p.seg_start && p.seg_count), "segment pointers");
+  PNX_CHECK_ARG(p.B == 0 || (p.edge_start ? (p.e_det && p.e_box && p.e_dist) : p.edge_count != nullptr), "pair outputs");
   return PNX_OK;
 }
 
@@ -1193,15 +1399,16 @@ extern "C" int pnx_eval_mot(const int* edge_start, const int* edge_count, long l
                             const int* gt_obj, const int* gt_points, const int* seq_start, int S, int B, int M, int C,
                             int K, int n_obj, int cap, int* last_id, long long* counts, double* dist, void* workspace,
                             cudaStream_t stream) {
-  const MotArgs a{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, e_iou, det_pass, det_id, gt_obj,
-                  gt_points, seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, counts, dist, workspace};
+  const MotArgs a{{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, det_pass, det_id, gt_obj,
+                   seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, workspace},
+                  e_iou, gt_points, counts, dist};
   int rc = check_mot_args(a);
   if (rc) return rc;
   const long long rows = (long long)S * C * K;
   if (rows == 0) return PNX_OK;
   PNX_CHECK_ARG(workspace, "workspace");
   if (n_obj > 0) PNX_CUDA(cudaMemsetAsync(last_id, 0xff, (size_t)K * n_obj * sizeof(int), stream));
-  eval_mot_kernel<<<(unsigned)rows, 32, 0, stream>>>(a);
+  eval_mot_kernel<MotArgs, LevelCounts><<<(unsigned)rows, 32, 0, stream>>>(a);
   PNX_CHECK_LAUNCH();
   return PNX_OK;
 }
@@ -1211,16 +1418,82 @@ extern "C" int pnx_eval_mot_host(const int* edge_start, const int* edge_count, l
                                  const float* e_iou, long long n_det, const int* det_pass, const int* det_id,
                                  const int* gt_obj, const int* gt_points, const int* seq_start, int S, int B, int M,
                                  int C, int K, int n_obj, int cap, int* last_id, long long* counts, double* dist) {
-  const MotArgs a{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, e_iou, det_pass, det_id, gt_obj,
-                  gt_points, seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, counts, dist, nullptr};
+  const MotArgs a{{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, det_pass, det_id, gt_obj,
+                   seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, nullptr},
+                  e_iou, gt_points, counts, dist};
   int rc = check_mot_args(a);
   if (rc) return rc;
-  for (long long i = 0; i < (long long)K * n_obj; ++i) last_id[i] = -1;
-  char* ws = new char[mot_row_bytes(M, cap)];
-  int scal[2];
-  const CompMem m = workspace_mem(ws, cap, 0, scal);
-  for (long long row = 0; row < (long long)S * C * K; ++row)
-    mot_row(HostGroup{}, a, (int)row, m, (int*)(ws + mot_comp_bytes(cap)));
-  delete[] ws;
+  host_mot<MotArgs, LevelCounts>(a);
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_pairs_center(const float* det_boxes, long long n_det, const long long* order,
+                                     const int* seg_start, const int* seg_count, const float* gt_boxes,
+                                     const int* gt_classes, int B, int M, int C, double max_dist, const int* edge_start,
+                                     int* edge_count, int* e_det, int* e_box, float* e_dist, cudaStream_t stream) {
+  const CenterPairArgs p{det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, B, M, C, max_dist, n_det,
+                         edge_start, edge_count, e_det, e_box, e_dist};
+  int rc = check_pairs_center_args(p);
+  if (rc) return rc;
+  if (B == 0) return PNX_OK;
+  const size_t smem = (size_t)M * (2 * sizeof(float) + sizeof(int));
+  eval_pairs_center_kernel<<<B * C, 32, smem, stream>>>(p);    // at most 48 KB: M <= 4096
+  PNX_CHECK_LAUNCH();
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_pairs_center_host(const float* det_boxes, long long n_det, const long long* order,
+                                          const int* seg_start, const int* seg_count, const float* gt_boxes,
+                                          const int* gt_classes, int B, int M, int C, double max_dist,
+                                          const int* edge_start, int* edge_count, int* e_det, int* e_box,
+                                          float* e_dist) {
+  const CenterPairArgs p{det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, B, M, C, max_dist, n_det,
+                         edge_start, edge_count, e_det, e_box, e_dist};
+  int rc = check_pairs_center_args(p);
+  if (rc) return rc;
+  host_pairs_center(p);
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_mot_center(const int* edge_start, const int* edge_count, long long n_edges, const int* grouped,
+                                   const int* comp_start, const int* comp_nedge, const int* e_det, const int* e_box,
+                                   const float* e_dist, long long n_det, const int* det_pass, const int* det_id,
+                                   const int* gt_obj, const int* gt_prev, const int* seq_start, int S, int B, int M,
+                                   int C, int K, int n_obj, int cap, int* last_id, int* last_frame, long long* counts,
+                                   double* dist, unsigned char* matched, void* workspace, cudaStream_t stream) {
+  const CenterMotArgs a{{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, det_pass, det_id,
+                         gt_obj, seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, workspace},
+                        e_dist, gt_prev, last_frame, counts, dist, matched};
+  int rc = check_center_mot_args(a);
+  if (rc) return rc;
+  if (matched && n_det > 0) PNX_CUDA(cudaMemsetAsync(matched, 0, (size_t)n_det, stream));
+  const long long rows = (long long)S * C * K;
+  if (rows == 0) return PNX_OK;
+  PNX_CHECK_ARG(workspace, "workspace");
+  if (n_obj > 0) {
+    PNX_CUDA(cudaMemsetAsync(last_id, 0xff, (size_t)K * n_obj * sizeof(int), stream));
+    PNX_CUDA(cudaMemsetAsync(last_frame, 0xff, (size_t)K * n_obj * sizeof(int), stream));
+  }
+  eval_mot_kernel<CenterMotArgs, CenterCounts><<<(unsigned)rows, 32, 0, stream>>>(a);
+  PNX_CHECK_LAUNCH();
+  return PNX_OK;
+}
+
+extern "C" int pnx_eval_mot_center_host(const int* edge_start, const int* edge_count, long long n_edges,
+                                        const int* grouped, const int* comp_start, const int* comp_nedge,
+                                        const int* e_det, const int* e_box, const float* e_dist, long long n_det,
+                                        const int* det_pass, const int* det_id, const int* gt_obj, const int* gt_prev,
+                                        const int* seq_start, int S, int B, int M, int C, int K, int n_obj, int cap,
+                                        int* last_id, int* last_frame, long long* counts, double* dist,
+                                        unsigned char* matched) {
+  const CenterMotArgs a{{edge_start, edge_count, grouped, comp_start, comp_nedge, e_det, e_box, det_pass, det_id,
+                         gt_obj, seq_start, S, B, M, C, K, n_obj, cap, n_edges, n_det, last_id, nullptr},
+                        e_dist, gt_prev, last_frame, counts, dist, matched};
+  int rc = check_center_mot_args(a);
+  if (rc) return rc;
+  if (matched)
+    for (long long i = 0; i < n_det; ++i) matched[i] = 0;
+  for (long long i = 0; i < (long long)K * n_obj; ++i) last_frame[i] = -1;
+  host_mot<CenterMotArgs, CenterCounts>(a);
   return PNX_OK;
 }

@@ -123,8 +123,9 @@ def _radius(boxes):
 
 
 def pack(gts, detections, class_names, class_range=None):
-    """gts / detections as for nuscenes_metrics -> filtered, keyed and segmented flat arrays (numpy, host).  The point
-    filter waits for the counts (run_device / run_host): gt_classes has the range filter applied only."""
+    """gts / detections as for nuscenes_metrics -> filtered, keyed and segmented flat arrays (numpy, host); det_pos =
+    each kept detection's position in the detections concatenated in the order of `detections`.  The point filter
+    waits for the counts (run_device / run_host): gt_classes has the range filter applied only."""
     rng = class_ranges(class_names, class_range)
     tokens = list(gts)
     frame_of = {t: f for f, t in enumerate(tokens)}
@@ -203,7 +204,7 @@ def pack(gts, detections, class_names, class_range=None):
     seg_count = np.bincount(seg, minlength=B * C).astype(np.int32)
     return dict(B=B, M=M, C=C, class_names=list(class_names), gt_boxes=gt_boxes, gt_classes=gt_classes, gt_attr=gt_attr,
                 num_points=known, points=points, det_boxes=np.ascontiguousarray(det_boxes), det_scores=det_scores,
-                det_labels=det_labels, det_frames=det_frames,
+                det_labels=det_labels, det_frames=det_frames, det_pos=det_pos,
                 det_attr=derive_attributes(det_labels, det_boxes[:, 6:8], class_names, vocab),
                 order=np.lexsort((-det_pos, -score64, seg)).astype(np.int64),
                 visit=np.lexsort((-det_pos, -score64, det_labels)).astype(np.int64),

@@ -1516,3 +1516,100 @@ def eval_mot_host(edge_start, e_det, e_box, e_iou, grouped, comp_start, comp_ned
                                   *[_hp(t) for t in ops_[7:]], S, B, int(M), C, int(K), int(n_obj), cap,
                                   _hp(last_id), _hp(counts), _hp(dist)))
     return counts, dist
+
+
+# --------------------------------------------------------------------------------- nuScenes tracking
+def _eval_pairs_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, host=False):
+    D, C = len(det_boxes), int(n_classes)
+    B, M = gt_boxes.shape[:2] if gt_boxes.ndim == 3 else (0, 0)
+    f32, i32 = torch.float32, torch.int32
+    return [_want(t, dtype, shape, what, host) for t, dtype, shape, what in (
+        (det_boxes, f32, (D, 9), "det_boxes"), (order, torch.int64, (D,), "order"),
+        (seg_start, i32, (B * C,), "seg_start"), (seg_count, i32, (B * C,), "seg_count"),
+        (gt_boxes, f32, (B, M, 9), "gt_boxes"), (gt_classes, i32, (B, M), "gt_classes"))]
+
+
+def eval_pairs_center(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, max_dist):
+    """The pairs of every (frame, class) segment with centre distance < max_dist (pnx_eval_pairs_center,
+    include/pnx.h), operands as for eval_match_center, all CUDA -> (edge_start [B C] int32, e_det [E] int32, e_box [E]
+    int32 f M + j, e_dist [E] fp32).  One count pass, one prefix sum, one host read of E, one write pass."""
+    db, od, ss, sc, gb, gc = _eval_pairs_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes,
+                                                         n_classes)
+    D, (B, M), C = len(db), gb.shape[:2], int(n_classes)
+    dev = db.device
+    count = torch.zeros(B * C, dtype=torch.int32, device=dev)
+    args = (ptr(db), D, ptr(od), ptr(ss), ptr(sc), ptr(gb), ptr(gc), B, M, C, float(max_dist))
+    _count(2)
+    check(lib().pnx_eval_pairs_center(*args, None, ptr(count), None, None, None, stream()))
+    end = torch.cumsum(count, 0, dtype=torch.int64)
+    E = int(end[-1]) if B * C else 0
+    start = (end - count).to(torch.int32)
+    e_det, e_box = (torch.empty(E, dtype=torch.int32, device=dev) for _ in range(2))
+    e_dist = torch.empty(E, dtype=torch.float32, device=dev)
+    if E:
+        check(lib().pnx_eval_pairs_center(*args, ptr(start), ptr(count), ptr(e_det), ptr(e_box), ptr(e_dist), stream()))
+    return start, e_det, e_box, e_dist
+
+
+def eval_pairs_center_host(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes, n_classes, max_dist):
+    """Host twin of eval_pairs_center (pnx_eval_pairs_center_host): numpy in -> the same four arrays."""
+    db, od, ss, sc, gb, gc = _eval_pairs_center_operands(det_boxes, order, seg_start, seg_count, gt_boxes, gt_classes,
+                                                         n_classes, host=True)
+    D, (B, M), C = len(db), gb.shape[:2], int(n_classes)
+    count = np.zeros(B * C, np.int32)
+    args = (_hp(db), D, _hp(od), _hp(ss), _hp(sc), _hp(gb), _hp(gc), B, M, C, float(max_dist))
+    check(lib().pnx_eval_pairs_center_host(*args, None, _hp(count), None, None, None))
+    start = (np.cumsum(count, dtype=np.int64) - count).astype(np.int32)
+    E = int(count.sum(dtype=np.int64))
+    e_det, e_box, e_dist = np.zeros(E, np.int32), np.zeros(E, np.int32), np.zeros(E, np.float32)
+    if E:
+        check(lib().pnx_eval_pairs_center_host(*args, _hp(start), _hp(count), _hp(e_det), _hp(e_box), _hp(e_dist)))
+    return start, e_det, e_box, e_dist
+
+
+def eval_mot_center(edge_start, e_det, e_box, e_dist, grouped, comp_start, comp_nedge, det_pass, det_id, gt_obj,
+                    gt_prev, seq_start, M, n_classes, K, n_obj, want_matched=False):
+    """nuScenes tracking's frame matching per (scene, class, cutoff) (pnx_eval_mot_center, include/pnx.h), all CUDA:
+    the pairs of eval_pairs_center, the components of eval_components, det_pass / det_id [D] int32, gt_obj / gt_prev
+    [B M] int32, seq_start [S + 1] int32 -> (counts [S, C, K, 3] int64 matches / identity switches / fragmentations,
+    dist [S, C, K] fp64, matched [D] uint8 or None).  want_matched needs K = 1.  The workspace is eval_mot's: every
+    (scene, class, cutoff) row gets 164 B per pair of the largest component anywhere plus 4 B per box slot, S C K (164
+    cap + 4 M) bytes (nuScenes val shape, 150 x 7 x 40 = 42,000 rows: a largest component of 159 pairs takes 1.1 GB; it
+    grows linearly with the densest crowd of detections, 14 GB at 2000 pairs)."""
+    ops_ = _eval_mot_operands(edge_start, e_det, e_box, e_dist, grouped, comp_start, comp_nedge, det_pass, det_id,
+                              gt_obj, gt_prev, seq_start)
+    st = ops_[0]
+    E, D, S, C, B = len(ops_[4]), len(ops_[7]), len(ops_[11]) - 1, int(n_classes), len(st) // int(n_classes)
+    dev = st.device
+    cap = _mot_cap(ops_[3])
+    count = _edge_count(st, E)
+    counts = torch.empty((S, C, int(K), 3), dtype=torch.int64, device=dev)
+    dist = torch.empty((S, C, int(K)), dtype=torch.float64, device=dev)
+    last_id, last_frame = (torch.empty(max(1, int(K) * int(n_obj)), dtype=torch.int32, device=dev) for _ in range(2))
+    matched = torch.empty(D, dtype=torch.uint8, device=dev) if want_matched else None
+    ws = torch.empty(max(1, lib().pnx_eval_mot_workspace(S * C * int(K), int(M), cap)), dtype=torch.uint8, device=dev)
+    _count(1)
+    check(lib().pnx_eval_mot_center(ptr(st), ptr(count), E, *[ptr(t) for t in ops_[1:7]], D,
+                                    *[ptr(t) for t in ops_[7:]], S, B, int(M), C, int(K), int(n_obj), cap,
+                                    ptr(last_id), ptr(last_frame), ptr(counts), ptr(dist), ptr(matched), ptr(ws),
+                                    stream()))
+    return counts, dist, matched
+
+
+def eval_mot_center_host(edge_start, e_det, e_box, e_dist, grouped, comp_start, comp_nedge, det_pass, det_id, gt_obj,
+                         gt_prev, seq_start, M, n_classes, K, n_obj, want_matched=False):
+    """Host twin of eval_mot_center (pnx_eval_mot_center_host): numpy in -> (counts, dist, matched or None)."""
+    ops_ = _eval_mot_operands(edge_start, e_det, e_box, e_dist, grouped, comp_start, comp_nedge, det_pass, det_id,
+                              gt_obj, gt_prev, seq_start, host=True)
+    st = ops_[0]
+    E, D, S, C, B = len(ops_[4]), len(ops_[7]), len(ops_[11]) - 1, int(n_classes), len(st) // int(n_classes)
+    cap = _mot_cap(ops_[3])
+    count = _edge_count(st, E)
+    counts, dist = np.zeros((S, C, int(K), 3), np.int64), np.zeros((S, C, int(K)), np.float64)
+    last_id, last_frame = (np.zeros(max(1, int(K) * int(n_obj)), np.int32) for _ in range(2))
+    matched = np.zeros(D, np.uint8) if want_matched else None
+    check(lib().pnx_eval_mot_center_host(_hp(st), _hp(count), E, *[_hp(t) for t in ops_[1:7]], D,
+                                         *[_hp(t) for t in ops_[7:]], S, B, int(M), C, int(K), int(n_obj), cap,
+                                         _hp(last_id), _hp(last_frame), _hp(counts), _hp(dist),
+                                         None if matched is None else _hp(matched)))
+    return counts, dist, matched

@@ -146,22 +146,23 @@ def make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=0.05, ego_speed=5.0
     return pts[order], T, owner[order]
 
 
-SEQUENCE_STEP_US = 100000           # frames of a sequence are 0.1 s apart
+SEQUENCE_STEP_US = 100000           # default: frames of a sequence are 0.1 s apart
 SEQUENCE_T0_US = 1000000000         # timestamp of every sequence's first frame
 
 
-def sequence_frame(seed, k, cfg, n_points=6000, n_boxes=12, ego_speed=5.0):
-    """Frame k >= 0 of the sequence that starts with make_scene(seed): the scene k * 0.1 s later, with make_sweep's
-    motion run forward (each box at centre + v * 0.1 k, the ego on ego_pose's arc), scanned from the ego's pose then.
+def sequence_frame(seed, k, cfg, n_points=6000, n_boxes=12, ego_speed=5.0, step_us=SEQUENCE_STEP_US):
+    """Frame k >= 0 of the sequence that starts with make_scene(seed): the scene k * dt later (dt = step_us * 1e-6 s),
+    with make_sweep's motion run forward (each box at centre + v dt k, the ego on ego_pose's arc), scanned from the
+    ego's pose then.
     Returns (points [N, 5] fp32 with time 0, boxes [M, 9] fp32 in frame k's sensor frame -- velocity rotated into it,
     the order and so the object ids of make_scene's boxes --, names, pose [4, 4] fp64 frame k's sensor -> the first
     frame's sensor).  Frame 0 is exactly make_scene(seed) with the identity pose."""
     pts, boxes, names = make_scene(seed, cfg, n_points, n_boxes)
     if k == 0:
         return pts, boxes, names, np.eye(4)
-    p, T, _ = make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=-SEQUENCE_STEP_US * 1e-6, ego_speed=ego_speed)
+    p, T, _ = make_sweep(seed, k, cfg, boxes, n_points, sweep_interval=-step_us * 1e-6, ego_speed=ego_speed)
     p[:, 4] = 0.0
-    lag = k * -SEQUENCE_STEP_US * 1e-6                              # make_sweep's box motion, and the velocity
+    lag = k * -step_us * 1e-6                              # make_sweep's box motion, and the velocity
     b = boxes.astype(np.float64).copy()
     b[:, :2] -= b[:, 6:8] * lag
     R, t = T[:2, :2], T[:2, 3]
@@ -191,7 +192,7 @@ def sampling_record(sampler, boxes, names, class_names):
             "scene_trig": numpy_trig(boxes)}
 
 
-METRICS = ("nuscenes", "waymo", "nds", "waymo_tracking")
+METRICS = ("nuscenes", "waymo", "nds", "waymo_tracking", "nds_tracking")
 
 
 class SyntheticSceneDataset(torch.utils.data.Dataset):
@@ -214,7 +215,8 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     takes the sweeps into the key frame on the GPU (ops.accumulate_sweeps), dropping the sweep points within
     min_distance of the sensor in x and y (nuScenes' remove_close; 0 = off).  nsweeps = 1 frames are unchanged.
 
-    sequence_length: frames are grouped into sequences of that many frames, 0.1 s apart (sequence_frame: sequence q
+    sequence_length, sequence_interval: frames are grouped into sequences of sequence_length frames, sequence_interval
+    seconds apart (default 0.1; nuScenes key frames are 0.5 s apart) (sequence_frame: sequence q
     starts with make_scene(seed0 + q L); its objects keep their ids and move by their velocity labels, the ego follows
     ego_pose).  Each frame's token is then "seq<seed>-<timestamp_micros>" and ground_truth() carries its sequence,
     timestamp, pose and the objects' ids.  The default 1 leaves every frame and token as they were.  Sequences do not
@@ -223,14 +225,17 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
     metric: what evaluation() reports -- "nuscenes" (evaluate.detection_map), "waymo" (evaluate_waymo.waymo_metrics,
     AP / APH at LEVEL_1 and LEVEL_2), "nds" (evaluate_nuscenes.nuscenes_metrics, the nuScenes detection score with
     its true-positive errors) or "waymo_tracking" (the "waymo" dict plus "tracking": the detections tracked by
-    track.track and scored by evaluate_waymo_tracking.waymo_tracking_metrics).  For every metric but "nuscenes"
+    track.track and scored by evaluate_waymo_tracking.waymo_tracking_metrics) or "nds_tracking" (the "nds" dict plus
+    "tracking": evaluate_nuscenes_tracking.track_and_score's metrics; needs sequence_length > 1).  For every metric but
+    "nuscenes"
     ground_truth() also hands over each frame's points.
     waymo_matching: for metric "waymo", "greedy" (the default) or "hungarian" (the maximum-IoU matching at score-cutoff
     quantiles with the range breakdown, evaluate_waymo.py)."""
 
     def __init__(self, cfg, n_frames, seed0=0, n_points=6000, n_boxes=12, test_mode=False, class_names=None,
                  augmentation=None, sampler=None, root_path=None, metric="nuscenes", nsweeps=1, drop_frames=0.0,
-                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, waymo_matching="greedy", sequence_length=1, **_):
+                 sweep_interval=0.05, ego_speed=5.0, min_distance=1.0, waymo_matching="greedy", sequence_length=1,
+                 sequence_interval=0.1, **_):
         if int(nsweeps) < 1 or not 0.0 <= drop_frames <= 1.0 or min_distance < 0:
             raise ValueError("nsweeps must be >= 1, drop_frames in [0, 1] and min_distance >= 0, got %r, %r, %r"
                              % (nsweeps, drop_frames, min_distance))
@@ -243,6 +248,11 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
         self.sequence_length = int(sequence_length)
         if self.sequence_length < 1 or (self.sequence_length > 1 and self.nsweeps > 1):
             raise ValueError("sequence_length must be >= 1, and 1 when nsweeps > 1, got %r" % (sequence_length,))
+        self.sequence_step_us = int(round(float(sequence_interval) * 1e6))
+        if self.sequence_step_us <= 0:
+            raise ValueError("sequence_interval must be > 0 seconds, got %r" % (sequence_interval,))
+        if metric == "nds_tracking" and self.sequence_length < 2:
+            raise ValueError("metric nds_tracking needs sequences: sequence_length >= 2")
         self.metric = metric
         from .evaluate_waymo import check_matching
         self.waymo_matching = check_matching(waymo_matching)
@@ -267,8 +277,9 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
             return pts, boxes, names, "scene_%d" % (self.seed0 + i), None, None, None
         q, k = divmod(i, self.sequence_length)
         seed = self.seed0 + q * self.sequence_length
-        pts, boxes, names, pose = sequence_frame(seed, k, self.cfg, self.n_points, self.n_boxes, self.ego_speed)
-        ts = SEQUENCE_T0_US + k * SEQUENCE_STEP_US
+        pts, boxes, names, pose = sequence_frame(seed, k, self.cfg, self.n_points, self.n_boxes, self.ego_speed,
+                                                 self.sequence_step_us)
+        ts = SEQUENCE_T0_US + k * self.sequence_step_us
         return pts, boxes, names, "seq%d-%d" % (seed, ts), "seq%d" % seed, ts, pose
 
     def __getitem__(self, i):
@@ -322,9 +333,14 @@ class SyntheticSceneDataset(torch.utils.data.Dataset):
                 from .evaluate_waymo_tracking import track_and_score
                 res["tracking"] = track_and_score(gts, detections, self.class_names)[1]
             return res
-        if self.metric == "nds":
+        if self.metric in ("nds", "nds_tracking"):
             from .evaluate_nuscenes import nuscenes_metrics
-            return nuscenes_metrics(self.ground_truth(), detections, self.class_names)
+            gts = self.ground_truth()
+            res = nuscenes_metrics(gts, detections, self.class_names)
+            if self.metric == "nds_tracking":
+                from .evaluate_nuscenes_tracking import track_and_score
+                res["tracking"] = track_and_score(gts, detections, self.class_names)[1]
+            return res
         from .evaluate import detection_map
         return detection_map(self.ground_truth(), detections, self.class_names)
 

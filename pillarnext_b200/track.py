@@ -20,8 +20,11 @@ reference.  It is the consumer of the CenterHead's velocity output (`vel`).
     seen again starts a new track.
   * Ids: consecutive integers per sequence, from 0, in order of birth (frame, then class index, then visit order).
     Detections below min_score get tracking id -1 and neither start nor continue a track.
-  * Defaults: max_dist vehicle 2.0 m, pedestrian 1.0 m, cyclist 1.5 m.  These are this project's choice, not values
-    taken from CenterPoint's released tracker.  A class outside that table needs an entry in max_dist.
+  * Defaults: max_dist vehicle 2.0 m, pedestrian 1.0 m, cyclist 1.5 m (MAX_DIST, Waymo's classes at 10 Hz).  A class
+    outside that table needs an entry in max_dist.  NUSCENES_MAX_DIST holds the entries for nuScenes' tracking classes
+    at its 2 Hz key frames, where the velocity back-projection spans 0.5 s: car 4.0 m, truck 4.0 m, bus 5.0 m, trailer
+    3.0 m, motorcycle 4.0 m, bicycle 2.5 m, pedestrian 1.0 m; evaluate_nuscenes_tracking.track_and_score passes them.
+    All of these are this project's choice, not values taken from CenterPoint's released tracker.
 
 At most 4096 tracks (pnx_track_max_tracks()) of one (sequence, class) may be live at once, counting those born in the
 current frame; more raise ValueError.  The tracker runs on the GPU (pnx_track_greedy, csrc/track.cu: one warp per
@@ -31,6 +34,8 @@ import numpy as np
 import torch
 
 MAX_DIST = {"vehicle": 2.0, "pedestrian": 1.0, "cyclist": 1.5}
+NUSCENES_MAX_DIST = {"car": 4.0, "truck": 4.0, "bus": 5.0, "trailer": 3.0, "motorcycle": 4.0, "bicycle": 2.5,
+                     "pedestrian": 1.0}
 
 
 def split_token(token):
